@@ -94,7 +94,11 @@ typedef struct rn_config {
 
   /* stepSizeTuner(): DualAvgTuner(delta) DualAvg.scala:3 | StaticStepSize(stepSize) Sampler.scala:36-40 */
   int32_t step_size_tuner;   /* RN_STEP_* */
-  int32_t reserved1;
+  int32_t step_adaptation;   /* extension: RN_ADAPT_PER_CHAIN (parity with the reference, default) or RN_ADAPT_POOLED:
+                                one DualAvg state shared by all chains (and, when a communicator is attached, all
+                                ranks), started at 2^(mean log2 of the chains' findReasonableStepSize) and updated
+                                every warmup iteration with the chains' mean acceptance probability (exact integer
+                                sums, DESIGN.md §3.2).  Independent of `adaptation`; needs DualAvgTuner */
   double delta;              /* default 0.8 */
   double static_step_size;
 

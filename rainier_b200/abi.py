@@ -36,7 +36,7 @@ class Config(C.Structure):
         ("backend", C.c_int32),
         ("p_count", C.c_double),
         ("step_size_tuner", C.c_int32),
-        ("reserved1", C.c_int32),
+        ("step_adaptation", C.c_int32),
         ("delta", C.c_double),
         ("static_step_size", C.c_double),
         ("mass_tuner", C.c_int32),

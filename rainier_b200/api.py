@@ -253,6 +253,7 @@ class SamplerConfig:
     mathMode = abi.RN_MATH_PARITY
     gradientMode = abi.RN_GRAD_AUTO
     adaptation = abi.RN_ADAPT_PER_CHAIN
+    stepAdaptation = abi.RN_ADAPT_PER_CHAIN  # RN_ADAPT_POOLED: one DualAvg step size fitted to all chains' mean acceptance
     launchIterations = 0
     backend = abi.RN_BACKEND_AUTO
 
@@ -317,6 +318,7 @@ def lower_config(config):
         raise RainierCudaError(abi.RN_E_UNSUPPORTED, "unknown MassMatrixTuner")
     c.math_mode, c.gradient_mode = int(config.mathMode), int(config.gradientMode)
     c.adaptation, c.launch_iterations = int(config.adaptation), int(config.launchIterations)
+    c.step_adaptation = int(config.stepAdaptation)
     c.backend = int(config.backend)
     return c, keep
 

@@ -54,6 +54,10 @@ struct RnArgs {
   int chain_begin;               // rn_k_iter works on chains [chain_begin, chain_end): rn_sample pipelines chain blocks
   int chain_end;                 //   against the device->host copy of the previous block
   int pad1;
+  // pooled step-size adaptation (RN_STEP_POOL modules only, rn_step_pool.cuh): rn_k_init adds into step_acc[0] (sum of
+  // the chains' log2 initial step sizes) and step_acc[1] (chains); a warmup launch of one iteration adds its quantised
+  // acceptance probabilities into *step_acc (the slot of that iteration)
+  rn_i64* step_acc;
 };
 
 // argument block of rn_k_eval (rn_function.cuh): batched evaluation of a compiled function, generic addressing

@@ -16,6 +16,8 @@ namespace rn {
 extern const char* kPreludeSource;  // rn_prelude.cuh, embedded at build time
 extern const char* kSamplerSource;     // rn_args.h + rn_sampler.cuh
 extern const char* kSamplerWpcSource;  // rn_args.h + rn_sampler_wpc.cuh
+extern const char* kStepPoolSource;       // rn_step_pool.cuh (RN_STEP_POOL modules)
+extern const char* kStepPoolApplySource;  // rn_step_pool_apply.cuh (RN_STEP_POOL modules)
 extern const char* kFunctionSource;    // rn_function.cuh
 extern const char* kOptimizerSource;   // rn_args.h + rn_optimizer.cuh
 
@@ -1875,6 +1877,7 @@ std::string emit_source(const Program& P, const EmitOptions& opt) {
   os << "#define RN_BACKEND " << opt.backend << "\n";
   os << "#define RN_MASS_MAX " << opt.mass_max << "\n";
   os << "#define RN_ENABLE_EHMC " << (opt.enable_ehmc ? 1 : 0) << "\n";
+  if (opt.step_pool) os << "#define RN_STEP_POOL 1\n";
   if (opt.fast_math) os << "#define RN_FAST_MATH 1\n";
   if (opt.backend == 1) {
     os << "#define RN_WPC_K " << std::max(1, opt.wpc_k) << "\n";
@@ -1885,6 +1888,7 @@ std::string emit_source(const Program& P, const EmitOptions& opt) {
     }
   }
   os << kPreludeSource << "\n";
+  if (opt.step_pool) os << kStepPoolSource << "\n";
   if (opt.backend == 1)  // (RN_WPC_SCRATCH is defined by the emitted density; macros expand where they are used)
     os << "#define RN_WPC_SMEM_DOUBLES (" << wpc_vectors(opt) << " * RN_N + RN_WPC_SCRATCH)\n";
   os << emit_density(P, opt) << "\n";
@@ -1893,6 +1897,7 @@ std::string emit_source(const Program& P, const EmitOptions& opt) {
   } else {
     os << kSamplerSource << "\n";
   }
+  if (opt.step_pool) os << kStepPoolApplySource << "\n";
   return os.str();
 }
 

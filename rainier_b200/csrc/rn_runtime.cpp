@@ -155,8 +155,10 @@ struct KernelKey {
   bool adjoint, fast, ehmc;
   int mass_max, backend;
   int block = 0;  // thread-per-chain: CTA size the module was compiled for (RN_BLOCK_DIM), 0 = any (emit / density-only uses)
+  bool step_pool = false;  // pooled step-size adaptation compiled in (RN_STEP_POOL)
   bool operator<(const KernelKey& o) const {
-    return std::tie(adjoint, fast, ehmc, mass_max, backend, block) < std::tie(o.adjoint, o.fast, o.ehmc, o.mass_max, o.backend, o.block);
+    return std::tie(adjoint, fast, ehmc, mass_max, backend, block, step_pool) <
+           std::tie(o.adjoint, o.fast, o.ehmc, o.mass_max, o.backend, o.block, o.step_pool);
   }
 };
 // SMs of a device; handles without one (emit / compile only) assume an H100 SXM's 132
@@ -183,9 +185,10 @@ struct Kernel {
   std::vector<char> cubin;
   CUmodule mod = nullptr;
   CUfunction k_init = nullptr, k_iter = nullptr, k_warmup = nullptr, k_density = nullptr, k_transpose = nullptr, k_pool_reduce = nullptr,
-             k_pool_apply = nullptr, k_diag_chain = nullptr, k_diag_reduce = nullptr;
+             k_pool_apply = nullptr, k_diag_chain = nullptr, k_diag_reduce = nullptr, k_step_pool = nullptr;
   const Program* prog = nullptr;
   int backend = 0;            // 0 thread per chain, 1 warp per chain
+  bool step_pool = false;     // rn_k_step_pool compiled in (pooled step-size adaptation)
   unsigned tpc_block = 0;     // backend 0: the CTA size this module was compiled for (0: reads blockDim.x)
   int wpc_smem_doubles = 0;   // per-warp dynamic shared memory (backend 1)
   int warps_per_cta = 4;      // backend 1: CHAINS per CTA (each owned by wpc_k warps)
@@ -270,6 +273,7 @@ static KernelKey key_for(const rn_model* m, const rn_config* cfg) {
   k.adjoint = (gm == RN_GRAD_ADJOINT) || !m->rir_has_gradient;
   k.fast = cfg && cfg->math_mode == RN_MATH_FAST;
   k.ehmc = cfg && cfg->sampler == RN_SAMPLER_EHMC;
+  k.step_pool = cfg && cfg->step_adaptation == RN_ADAPT_POOLED;
   k.mass_max = 0;
   if (cfg) {
     if (cfg->mass_tuner == RN_MASS_DIAGONAL) k.mass_max = 1;
@@ -317,11 +321,13 @@ static int get_kernel(rn_model* m, const rn_config* cfg, Kernel** out, std::stri
   eo.fast_math = key.fast;
   eo.mass_max = key.mass_max;
   eo.enable_ehmc = key.ehmc;
+  eo.step_pool = key.step_pool;
   eo.target_base = m->target_base;
   eo.target_pitch = m->target_pitch;
   if (eo.backend == 1 && P->symbolic && P->n_params > 96)
     return fail(RN_E_UNSUPPORTED, "warp-per-chain with a symbolic gradient keeps n+1 accumulators in registers; use RN_GRAD_ADJOINT for n > 96");
   K->backend = eo.backend;
+  K->step_pool = key.step_pool;
   K->tpc_block = (unsigned)key.block;
   if (eo.backend == 0) {  // rn_sampler.cuh: RN_TS_DOUBLES * 8 + RN_TS_INTS * 4
     const unsigned n = P->n_params;
@@ -527,6 +533,7 @@ static int load_kernel(const Api* A, rn_model* m, Kernel* K) {
   CU(A->cuModuleGetFunction(&K->k_pool_apply, K->mod, "rn_k_pool_apply"));
   CU(A->cuModuleGetFunction(&K->k_diag_chain, K->mod, "rn_k_diag_chain"));
   CU(A->cuModuleGetFunction(&K->k_diag_reduce, K->mod, "rn_k_diag_reduce"));
+  if (K->step_pool) CU(A->cuModuleGetFunction(&K->k_step_pool, K->mod, "rn_k_step_pool"));
   if (K->backend == 1) {
     const int bytes = (int)K->smem_bytes();
     for (CUfunction f : {K->k_init, K->k_iter, K->k_density})
@@ -996,6 +1003,7 @@ struct rn_sampler {
   size_t trace_iters = 0, trace_pos = 0;
   rn_comm* comm = nullptr;
   CUdeviceptr d_pool = 0;  // [2n+1] pooled window statistics (RN_ADAPT_POOLED)
+  CUdeviceptr d_step = 0;  // int64 [2 + warmup]: K, C, Q_t of pooled step-size adaptation (rn_step_pool.cuh), zeroed at create
   // device time of the sampling phase (Stats.gradientTimes / iterationTimes, Stats.scala:8-9): events bracket every
   // batch of phase-1 launches; closed spans are summed when the stats are read
   CUevent ev_run[2] = {nullptr, nullptr};
@@ -1115,6 +1123,10 @@ int check_config(const rn_model* m, const rn_config* c, int chains) {
   }
   if (c->adaptation == RN_ADAPT_POOLED && c->mass_tuner != RN_MASS_DIAGONAL)
     return fail(RN_E_UNSUPPORTED, "pooled adaptation is implemented for the diagonal mass-matrix tuner");
+  if (c->step_adaptation != RN_ADAPT_PER_CHAIN && c->step_adaptation != RN_ADAPT_POOLED)
+    return fail(RN_E_INVALID, "step_adaptation must be RN_ADAPT_PER_CHAIN or RN_ADAPT_POOLED");
+  if (c->step_adaptation == RN_ADAPT_POOLED && c->step_size_tuner == RN_STEP_STATIC)
+    return fail(RN_E_UNSUPPORTED, "pooled step-size adaptation needs DualAvgTuner (a static step size has nothing to pool)");
   return RN_OK;
 }
 
@@ -1161,7 +1173,8 @@ int rn_sampler_create(rn_model* m, const rn_config* cfg, const int64_t* seeds, i
                o_chol = ar.take((dense ? n * (n + 1) / 2 : 0) * C * 8 + 8), o_emean = ar.take((diag ? n : 0) * C * 8 + 8),
                o_eraw = ar.take((diag ? n : 0) * C * 8 + 8), o_ecov = ar.take((dense ? n * n : 0) * C * 8 + 8),
                o_ring = ar.take((ehmc ? (size_t)cfg->buf_size : 0) * C * 8 + 8), o_ri = ar.take(C * 4), o_rf = ar.take(C * 4),
-               o_err = ar.take(C * 4);
+               o_err = ar.take(C * 4),
+               o_step = ar.take(cfg->step_adaptation == RN_ADAPT_POOLED ? (2 + (size_t)cfg->warmup_iterations) * 8 : 8);
   s->stats_off = ar.off;
   const size_t o_sg = ar.take(C * 8), o_ss = ar.take(C * 8), o_si = ar.take(C * 4), o_sa = ar.take(C * 4),
                o_se = ar.take(3 * C * 8), o_sen = ar.take(C * 4), o_sr = ar.take(3 * W * C * 8), o_sri = ar.take(3 * C * 4),
@@ -1201,6 +1214,8 @@ int rn_sampler_create(rn_model* m, const rn_config* cfg, const int64_t* seeds, i
   a.ring_i = (int*)P(o_ri);
   a.ring_full = (int*)P(o_rf);
   a.st_err = (int*)P(o_err);
+  s->d_step = s->arena + o_step;
+  a.step_acc = (rn_i64*)P(o_step);
   a.st_grads = (rn_i64*)P(o_sg);
   a.st_steps = (rn_i64*)P(o_ss);
   a.st_iters = (int*)P(o_si);
@@ -1293,15 +1308,32 @@ int rn_sampler_read_trace(rn_sampler* s, double* out /*[chains][iters][4]*/) {
   return RN_OK;
 }
 
+// in-place ncclAllReduce(sum) of `count` elements on the sampler's stream over the attached communicator (no-op without one
+// or with one rank); counted, and timed by event pairs, for rn_sampler_comm_stats
+static int comm_allreduce(const Api* A, rn_sampler* s, CUdeviceptr buf, size_t count, int nccl_type) {
+  if (!s->comm || s->comm->world <= 1) return RN_OK;
+  std::string why;
+  const Nccl* N = nccl(&why);
+  if (!N) return fail(RN_E_NCCL, why);
+  CUevent e0 = nullptr, e1 = nullptr;
+  if (s->allreduce_events.size() < 4096) {  // (pooled steps: one call per warmup iteration)
+    CU(A->cuEventCreate(&e0, 0));
+    CU(A->cuEventCreate(&e1, 0));
+    CU(A->cuEventRecord(e0, s->stream));
+  }
+  int r = N->AllReduce((const void*)(uintptr_t)buf, (void*)(uintptr_t)buf, count, nccl_type, 0 /*ncclSum*/, s->comm->comm, (void*)s->stream);
+  if (e1) {
+    A->cuEventRecord(e1, s->stream);
+    s->allreduce_events.push_back({e0, e1});
+  }
+  if (r != 0) return fail(RN_E_NCCL, std::string("ncclAllReduce: ") + (N->GetErrorString ? N->GetErrorString(r) : "?"));
+  s->allreduce_calls++;
+  return RN_OK;
+}
+
 static int pool_window(const Api* A, rn_sampler* s, int window_len) {
   const size_t n = s->m->n_params;
   CU(A->cuMemsetD8Async(s->d_pool, 0, (2 * n + 1) * 8, s->stream));
-  std::string why;
-  const Nccl* N = nullptr;
-  if (s->comm && s->comm->world > 1) {
-    N = nccl(&why);
-    if (!N) return fail(RN_E_NCCL, why);
-  }
   // two passes (pooled mean, then Chan's combination of the chains' M2 around it), each a deterministic reduction over this
   // GPU's chains followed by one small all-reduce over the ranks
   for (int pass = 0; pass < 2; pass++) {
@@ -1310,24 +1342,9 @@ static int pool_window(const Api* A, rn_sampler* s, int window_len) {
     void* params[] = {&s->args, &pool, &wl, &ps};
     CU(A->cuLaunchKernel(s->K->k_pool_reduce, (unsigned)n, 1, 1, 256, 1, 1, 0, s->stream, params, nullptr));
     s->launches++;
-    if (N) {
-      CUevent e0 = nullptr, e1 = nullptr;
-      if (s->allreduce_events.size() < 256) {
-        CU(A->cuEventCreate(&e0, 0));
-        CU(A->cuEventCreate(&e1, 0));
-        CU(A->cuEventRecord(e0, s->stream));
-      }
-      const CUdeviceptr buf = pass ? s->d_pool + (1 + n) * 8 : s->d_pool;
-      const size_t count = pass ? n : n + 1;
-      int r = N->AllReduce((const void*)(uintptr_t)buf, (void*)(uintptr_t)buf, count, 8 /*ncclFloat64*/, 0 /*ncclSum*/, s->comm->comm,
-                           (void*)s->stream);
-      if (e1) {
-        A->cuEventRecord(e1, s->stream);
-        s->allreduce_events.push_back({e0, e1});
-      }
-      if (r != 0) return fail(RN_E_NCCL, std::string("ncclAllReduce: ") + (N->GetErrorString ? N->GetErrorString(r) : "?"));
-      s->allreduce_calls++;
-    }
+    const int rc = pass ? comm_allreduce(A, s, s->d_pool + (1 + n) * 8, n, 8 /*ncclFloat64*/)
+                        : comm_allreduce(A, s, s->d_pool, n + 1, 8 /*ncclFloat64*/);
+    if (rc) return rc;
   }
   {
     CUdeviceptr pool = s->d_pool;
@@ -1339,11 +1356,24 @@ static int pool_window(const Api* A, rn_sampler* s, int window_len) {
   return RN_OK;
 }
 
+// pooled step-size adaptation (rn_step_pool.cuh): all-reduce the int64 sums of slot `slot` (.. + count) over the ranks, then
+// rn_k_step_pool(t, reset) on every chain
+static int step_pool_apply(const Api* A, rn_sampler* s, int slot, int count, int t, int reset) {
+  int rc = comm_allreduce(A, s, s->d_step + (size_t)slot * 8, (size_t)count, 4 /*ncclInt64*/);
+  if (rc) return rc;
+  CUdeviceptr acc = s->d_step;
+  void* params[] = {&s->args, &acc, &t, &reset};
+  CU(A->cuLaunchKernel(s->K->k_step_pool, (unsigned)((s->chains + 127) / 128), 1, 1, 128, 1, 1, 0, s->stream, params, nullptr));
+  s->launches++;
+  return RN_OK;
+}
+
 static int run_phase(const Api* A, rn_sampler* s, int phase, int iterations, double* d_samples, int chain_begin = 0,
                      int chain_end = -1) {
   if (chain_end < 0) chain_end = s->chains;
   const int per_launch = s->cfg.launch_iterations > 0 ? s->cfg.launch_iterations : 1000;
   const bool pooled = phase == 0 && s->cfg.adaptation == RN_ADAPT_POOLED && s->cfg.mass_tuner == RN_MASS_DIAGONAL;
+  const bool step_pooled = phase == 0 && s->K->step_pool;
   int done = 0;
   if (phase == 1 && iterations > 0) {
     if (!s->ev_run[0]) {
@@ -1359,7 +1389,10 @@ static int run_phase(const Api* A, rn_sampler* s, int phase, int iterations, dou
   while (done < iterations) {
     int k = std::min(per_launch, iterations - done);
     if (pooled) k = iterations_to_window_end(s, k);  // launches end exactly at window ends
+    if (step_pooled) k = 1;                          // every warmup iteration ends in a synchronisation over all chains
+    const int warm_t = s->warm_done + done;          // (phase 0) warmup iteration of this launch's first iteration
     RnArgs& a = s->args;
+    if (step_pooled) a.step_acc = (rn_i64*)(uintptr_t)(s->d_step + (2 + (size_t)warm_t) * 8);
     a.phase = phase;
     a.n_iter = k;
     a.adaptation = s->cfg.adaptation == RN_ADAPT_POOLED ? 1 : 0;
@@ -1395,6 +1428,12 @@ static int run_phase(const Api* A, rn_sampler* s, int phase, int iterations, dou
     }
     if (phase == 0) {
       const int closed = advance_window(s, k);
+      // Driver.scala:67-80 order: step update, mass update, stepSizeTuner.reset() -- the pooled mass window's reset is
+      // rn_k_pool_apply's, after this iteration's step update
+      if (step_pooled) {
+        rc = step_pool_apply(A, s, 2 + warm_t, 1, warm_t, (closed > 0 && !pooled) ? 1 : 0);
+        if (rc) return rc;
+      }
       if (pooled && closed > 0) {
         rc = pool_window(A, s, closed);
         if (rc) return rc;
@@ -1415,8 +1454,13 @@ int rn_sampler_warmup(rn_sampler* s, int iterations) {
   CU(A->cuCtxSetCurrent(s->m->ctx));
   if (!s->initialized) {
     s->args.mass_kind = 0;
+    s->args.step_acc = (rn_i64*)(uintptr_t)s->d_step;  // (pooled steps: K, C)
     int rc = launch(A, s, s->K->k_init);  // LeapFrog.initialize + tuner initialisation
     if (rc) return rc;
+    if (s->K->step_pool) {  // the shared DualAvg.apply(delta, 2^(K / C)) over all chains of all ranks
+      rc = step_pool_apply(A, s, 0, 2, -1, 0);
+      if (rc) return rc;
+    }
     s->initialized = true;
     if (s->cfg.mass_tuner == RN_MASS_STATIC) s->mass_kind = s->cfg.static_matrix;  // StaticMassMatrix.initialize
   }

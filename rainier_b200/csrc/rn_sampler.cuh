@@ -23,6 +23,9 @@
 // struct RnArgs: see rn_args.h (shared verbatim with the host runtime)
 
 #define RN_LN2 0.6931471805599453
+#ifndef RN_STEP_POOL
+#define RN_STEP_POOL 0 /* 1: pooled step-size adaptation (rn_step_pool.cuh, rn_step_pool_apply.cuh) */
+#endif
 #define RN_AT(ptr, field, c) (ptr)[(size_t)(field) * (size_t)A.chains + (size_t)(c)]
 
 // ---- this thread's COLD state lives in shared memory -----------------------------------------------------------
@@ -473,8 +476,14 @@ RN_GLOBAL void rn_k_init(const RnArgs A) {
     lap = rn_log_accept(rn_energy(A, c, T, s, 0, s.U) - H0);
     const double exponent = (lap > -RN_LN2) ? 1.0 : -1.0;
     const double doubleOrHalf = (exponent > 0) ? 2.0 : 0.5;
+#if RN_STEP_POOL
+    int log2Step = 0;  // stepSize == 2^log2Step (doubling / halving 1.0 is exact down to 0 = 2^-1075 and up to inf = 2^1024)
+#endif
     while (stepSize != 0.0 && (exponent * lap > -exponent * RN_LN2)) {
       stepSize *= doubleOrHalf;
+#if RN_STEP_POOL
+      log2Step += (exponent > 0) ? 1 : -1;
+#endif
       RN_UNROLL
       for (int i = 0; i < RN_N; i++) {
         RN_P(i) = RN_AT(A.params, i, c);
@@ -491,6 +500,11 @@ RN_GLOBAL void rn_k_init(const RnArgs A) {
     RN_AT(A.da, 3, c) = 0.0;
     RN_AT(A.da, 4, c) = rn_log(10 * stepSize);
     A.da_iter[c] = 0;
+#if RN_STEP_POOL
+    // pooled: K and C over all chains; rn_k_step_pool replaces this chain's DualAvg with the shared one
+    rn_pool_add(A.step_acc + 0, log2Step < -1075 ? -1075 : (log2Step > 1024 ? 1024 : log2Step));
+    rn_pool_add(A.step_acc + 1, 1);
+#endif
   } else {
     stepSize = A.static_step;
   }
@@ -726,6 +740,10 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
 
     if (PHASE == 0) {
       // ---------------- stepSizeTuner.update, Driver.scala:69 / DualAvg.scala:58-77 ----------------
+#if RN_STEP_POOL
+      // pooled: this chain's share of the iteration's acceptance sum; rn_k_step_pool applies the update (and any reset)
+      if (A.step_tuner == 0) rn_pool_add(A.step_acc + it, rn_pool_quantise(rn_exp(a)));
+#else
       if (A.step_tuner == 0) {
         const double newAcceptanceProb = rn_exp(a);
         const int daIter = A.da_iter[c] + 1;
@@ -739,6 +757,7 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
         RN_AT(A.da, 2, c) = (stepSizeMultiplier * logStepSize + (1.0 - stepSizeMultiplier) * RN_AT(A.da, 2, c));
         stepSize = rn_exp(logStepSize);
       }
+#endif
       // ---------------- massMatrixTuner.update(sample), Driver.scala:74-80 / MassMatrix.scala:147-164 -------
 #if RN_MASS_MAX >= 1
       if (A.mass_tuner == 1 || A.mass_tuner == 2) {
@@ -839,7 +858,8 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
                 }
             }
 #endif
-            // stepSize = stepSizeTuner.reset(), Driver.scala:78 / DualAvg.scala:17-21
+            // stepSize = stepSizeTuner.reset(), Driver.scala:78 / DualAvg.scala:17-21 (pooled steps: rn_k_step_pool)
+#if !RN_STEP_POOL
             if (A.step_tuner == 0) {
               const double ss = rn_exp(RN_AT(A.da, 2, c));
               RN_AT(A.da, 1, c) = rn_log(ss);
@@ -849,6 +869,7 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
               RN_AT(A.da, 4, c) = rn_log(10 * ss);
               stepSize = ss;
             }
+#endif
           }
         }
       }

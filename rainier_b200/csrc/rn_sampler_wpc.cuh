@@ -21,6 +21,9 @@
 #define RN_SAMPLER_WPC_CUH
 
 #define RN_LN2 0.6931471805599453
+#ifndef RN_STEP_POOL
+#define RN_STEP_POOL 0 /* 1: pooled step-size adaptation (rn_step_pool.cuh, rn_step_pool_apply.cuh) */
+#endif
 #define RN_AT(ptr, field, c) (ptr)[(size_t)(field) * (size_t)A.chains + (size_t)(c)]
 #define RN_LANE ((int)(threadIdx.x % RN_G))  // thread index inside the chain's group (RN_G, RN_SYNC: rn_prelude.cuh)
 #define RN_FOR_LANES(i) for (int i = RN_LANE; i < RN_N; i += RN_G)
@@ -309,8 +312,14 @@ RN_GLOBAL void rn_k_init(const RnArgs A) {
     double lap = rn_log_accept(rn_energy(w, w.p, w.U) - H0);
     const double exponent = (lap > -RN_LN2) ? 1.0 : -1.0;
     const double doubleOrHalf = (exponent > 0) ? 2.0 : 0.5;
+#if RN_STEP_POOL
+    int log2Step = 0;  // stepSize == 2^log2Step (see rn_sampler.cuh)
+#endif
     while (stepSize != 0.0 && (exponent * lap > -exponent * RN_LN2)) {
       stepSize *= doubleOrHalf;
+#if RN_STEP_POOL
+      log2Step += (exponent > 0) ? 1 : -1;
+#endif
       RN_SYNC();
       RN_FOR_LANES(i) {  // copy(params, pqBuf)
         w.p[i] = RN_AT(A.params, i, c);
@@ -328,6 +337,11 @@ RN_GLOBAL void rn_k_init(const RnArgs A) {
       RN_AT(A.da, 3, c) = 0.0;
       RN_AT(A.da, 4, c) = rn_log(10 * stepSize);
       A.da_iter[c] = 0;
+#if RN_STEP_POOL
+      // pooled: K and C over all chains, one lane per chain; rn_k_step_pool installs the shared DualAvg
+      rn_pool_add(A.step_acc + 0, log2Step < -1075 ? -1075 : (log2Step > 1024 ? 1024 : log2Step));
+      rn_pool_add(A.step_acc + 1, 1);
+#endif
     }
   } else {
     stepSize = A.static_step;
@@ -520,6 +534,10 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
     }
 
     if (A.phase == 0) {
+#if RN_STEP_POOL
+      // pooled: one lane per chain adds the chain's share of the iteration's acceptance sum; rn_k_step_pool applies the update
+      if (A.step_tuner == 0 && RN_LANE == 0) rn_pool_add(A.step_acc + it, rn_pool_quantise(rn_exp(a)));
+#else
       if (A.step_tuner == 0) {  // DualAvg.update, DualAvg.scala:58-77
         const double newAcceptanceProb = rn_exp(a);
         daIter = daIter + 1;
@@ -530,6 +548,7 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
         logStepSizeBar = (stepSizeMultiplier * logStepSize + (1.0 - stepSizeMultiplier) * logStepSizeBar);
         stepSize = rn_exp(logStepSize);
       }
+#endif
 #if RN_MASS_MAX >= 2
       if (A.mass_tuner == 2) {  // DenseMassMatrixTuner: WindowedMassMatrixTuner (MassMatrix.scala:147-164) over CovarianceEstimator
         win_j += 1;
@@ -599,7 +618,7 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
 #endif
             RN_SYNC();
             w.mass_kind = 2;
-            if (A.step_tuner == 0) {  // stepSizeTuner.reset(), DualAvg.scala:17-21
+            if (A.step_tuner == 0 && !RN_STEP_POOL) {  // stepSizeTuner.reset(), DualAvg.scala:17-21 (pooled: rn_k_step_pool)
               const double ss = rn_exp(logStepSizeBar);
               logStepSize = rn_log(ss);
               logStepSizeBar = 0.0;
@@ -656,7 +675,7 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
             win_i = 0;
             win_size = rn_d2i(win_size * A.win_expansion);
             w.mass_kind = 1;
-            if (A.step_tuner == 0) {  // stepSizeTuner.reset(), DualAvg.scala:17-21
+            if (A.step_tuner == 0 && !RN_STEP_POOL) {  // stepSizeTuner.reset(), DualAvg.scala:17-21 (pooled: rn_k_step_pool)
               const double ss = rn_exp(logStepSizeBar);
               logStepSize = rn_log(ss);
               logStepSizeBar = 0.0;

@@ -44,6 +44,24 @@ if rank == 0:
     print("pooled adaptation: identical mass matrix on all %d ranks:" % world, np.round(mass[0], 4))
 s.close()
 
+# pooled step sizes over NCCL: exact int64 sums, so N ranks x C/N chains reproduce 1 rank x C chains bit for bit
+cfgs = api.SamplerConfig(iterations=50, warmupIterations=300, stepAdaptation=abi.RN_ADAPT_POOLED)
+s = api.CudaSampler(model, cfgs, seeds=mine)
+s.set_comm(comm)
+d = torch.empty((50, model.nVars, len(mine)), dtype=torch.float64, device="cuda")
+s.warmup(-1)
+s.run(50, d.data_ptr())
+s.sync()
+calls, _ = s.comm_stats()
+full = rdist.gather_samples(d.permute(2, 0, 1).contiguous().cpu().numpy(), total)
+s.close()
+if rank == 0:
+    assert world == 1 or calls == cfgs.warmupIterations + 1, calls
+    ref = model.sample(cfgs, seeds=seeds)
+    assert np.array_equal(full, ref.chains), "pooled steps: sharded run differs from the single-GPU run"
+    print("pooled step sizes: %d ranks x %d chains == 1 rank x %d chains bit for bit; %d all-reduce calls"
+          % (world, total // world, total, calls))
+
 # BASELINE.json configs[3]: eight schools, DefaultConfig (EHMC + DualAvg + diagonal mass), 8192 chains over the ranks,
 # warmup with the pooled mass-matrix all-reduce (NCCL over NVLink); device-resident, timed on the device, max over ranks
 import time
