@@ -753,9 +753,11 @@ RN_GLOBAL void rn_k_transpose(const double* RN_RESTRICT src, double* RN_RESTRICT
 
 // =============================================================================================================
 // Pooled mass-matrix adaptation (RN_ADAPT_POOLED; an extension, not reference semantics): at a window end the
-// per-chain window sums {sum q_i, sum q_i^2} are reduced over all chains of this GPU into pool[1..2n] (pool[0] =
-// number of draws), all-reduced over ranks by the host (NCCL) and applied to every chain: one shared diagonal
-// mass matrix, sums cleared, DualAvg restarted from each chain's averaged step size (Driver.scala:75-80).
+// chains' Welford statistics of the window (mean_c, M2_c over L draws) are reduced over all chains of this GPU in two
+// passes -- pool[0] = number of chains and pool[1..n] = sum of the means, all-reduced over ranks by the host (NCCL),
+// then pool[n+1..2n] = sum of M2_c + L (mean_c - pooled mean)^2, all-reduced again -- and applied to every chain: one
+// shared diagonal mass matrix, statistics cleared, DualAvg restarted from each chain's averaged step size
+// (Driver.scala:75-80).
 // =============================================================================================================
 RN_GLOBAL void rn_k_pool_reduce(const RnArgs A, double* pool, int window_len, int pass) {
   // One block per parameter; thread t adds chains t, t + 256, ... in order, then a fixed tree: the result does not depend

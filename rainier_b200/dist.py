@@ -5,7 +5,8 @@ Chains are the unit of parallelism (each Driver.sample call owns its sampler, tu
 rainier-sampler/.../sampler/Driver.scala:13-17), so the sampling path needs NO collective: rank r runs the contiguous
 chain block `chain_block(total, r, world)` with the same per-chain seeds a single process would use, and results are
 rank-local until gathered.  The only exchange step is optional and warmup-only: pooling mass-matrix window statistics
-over all chains of all ranks (RN_ADAPT_POOLED) -- a sum all-reduce of {count, sum q_i, sum q_i^2} (2n+1 doubles).
+over all chains of all ranks (RN_ADAPT_POOLED) -- two sum all-reduces per window of the chains' Welford statistics: first
+{chains, sum of the chains' window means} (n+1 doubles), then sum of M2_c + L (mean_c - pooled mean)^2 (n doubles).
 
 torch.distributed is used purely as plumbing (NCCL on GPUs, gloo in the CPU tests).
 """
@@ -46,7 +47,8 @@ def combine_welford(n, mean, m2):
 
 
 def allreduce_window_stats(stats, group=None):
-    """stats: tensor [2n+1] = [count, s1(0..n-1), s2(0..n-1)] of this rank -> summed over all ranks (in place)"""
+    """stats: this rank's pooled-window buffer [2n+1] = [chains, sum of the chains' means (0..n-1), sum of M2_c +
+    L (mean_c - pooled mean)^2 (0..n-1)], or a slice of it -> summed over all ranks (in place)"""
     import torch.distributed as dist
     if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
         dist.all_reduce(stats, op=dist.ReduceOp.SUM, group=group)

@@ -1,13 +1,17 @@
 """
-Test infrastructure for pooled step-size adaptation (rn_config.step_adaptation == RN_ADAPT_POOLED): the oracle's lockstep
-restatement (tests/pooled_step_oracle.cpp, built on the unchanged per-chain oracle) and a host emulation of the runtime's
-per-iteration orchestration (one warmup launch per iteration, the iteration's int64 acceptance sum, rn_k_step_pool) over
-the kernel source the emitter produces.  Neither is part of the product.
+Test infrastructure for the pooled adaptation modes, pooled step sizes (rn_config.step_adaptation == RN_ADAPT_POOLED) and
+pooled mass windows (rn_config.adaptation == RN_ADAPT_POOLED): the oracle's lockstep restatement
+(tests/pooled_step_oracle.cpp, built on the unchanged per-chain oracle), a host emulation of the runtime's per-iteration
+orchestration of pooled steps (one warmup launch per iteration, the iteration's int64 acceptance sum, rn_k_step_pool) over
+the kernel source the emitter produces, and the pooled window variance three ways: rn_k_pool_reduce's summation order
+restated in float64 (`pool_reduce_restated`), exactly in rationals (`pooled_variance_exact`), and a first-order bound on
+the distance between the two (`pool_error_bound`, `welford_error_bound`).  None of it is part of the product.
 """
 import ctypes as C
 import hashlib
 import os
 import subprocess
+from fractions import Fraction
 
 import numpy as np
 
@@ -43,13 +47,15 @@ def _oracle_lib():
         L.rno_model_destroy.argtypes = [C.c_void_p]
         L.rno_model_nvars.argtypes = [C.c_void_p]
         L.rno_sample_pooled_step.argtypes = [C.c_void_p, C.POINTER(Config), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
-                                             C.c_void_p]
+                                             C.c_void_p, C.c_void_p, C.c_void_p]
         _ORACLE = L
     return _ORACLE
 
 
 def oracle_sample(rir, cols, cfg, seeds, dense_mass=False):
-    """the lockstep oracle: dict(samples [chains][iters][n], mass, stats (rn_chain_stats), trace [chains][warm+iters][4])"""
+    """the lockstep oracle: dict(samples [chains][iters][n], mass, stats (rn_chain_stats), trace [chains][warm+iters][4],
+    warm_draws [chains][warmup][n] = the position after every warmup iteration, window_mass [windows][n] = the pooled
+    variance of every closed window (pooled mass windows only))"""
     L = _oracle_lib()
     cols = [np.ascontiguousarray(c, dtype=np.float64) for c in cols]
     ptrs = (C.c_void_p * max(len(cols), 1))(*[c.ctypes.data for c in cols])
@@ -66,13 +72,16 @@ def oracle_sample(rir, cols, cfg, seeds, dense_mass=False):
         mass = np.zeros((chains, n * n if dense_mass else n))
         stats = (ChainStats * chains)()
         trace = np.zeros((chains, cfg.warmup_iterations + cfg.iterations, 4))
+        warm = np.zeros((chains, cfg.warmup_iterations, n))
+        win = np.zeros((max(len(window_closes(cfg)), 1), n))
         cfg.rng_states = None
         if L.rno_sample_pooled_step(h, C.byref(cfg), seeds.ctypes.data, chains, samples.ctypes.data, mass.ctypes.data,
-                                    C.cast(stats, C.c_void_p), trace.ctypes.data) != 0:
+                                    C.cast(stats, C.c_void_p), trace.ctypes.data, warm.ctypes.data, win.ctypes.data) != 0:
             raise RuntimeError(L.rno_last_error().decode())
     finally:
         L.rno_model_destroy(h)
-    return {"samples": samples, "mass": mass, "stats": stats, "trace": trace}
+    return {"samples": samples, "mass": mass, "stats": stats, "trace": trace, "warm_draws": warm,
+            "window_mass": win[:len(window_closes(cfg))]}
 
 
 _POOLED_SHIM = r"""
@@ -262,3 +271,181 @@ def window_closes(cfg):
             out.add(j - 1)
             i, size = 0, int(size * cfg.window_expansion)
     return out
+
+
+def windows(cfg):
+    """the warmup iterations (0-based) that make up every window WindowedMassMatrixTuner closes, in order"""
+    out, cur, size = [], [], cfg.initial_window_size
+    if cfg.mass_tuner not in (1, 2):
+        return out
+    for j in range(1, cfg.warmup_iterations + 1):
+        if j < cfg.skip_first or (cfg.warmup_iterations - j) < cfg.skip_last:
+            continue
+        cur.append(j - 1)
+        if len(cur) == size:
+            out.append(cur)
+            cur, size = [], int(size * cfg.window_expansion)
+    return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The pooled window variance of RN_ADAPT_POOLED (rn_k_pool_reduce, two passes around the pooled mean; rn_k_pool_apply)
+# ---------------------------------------------------------------------------------------------------------------------
+U = 2.0 ** -53     # unit roundoff of float64
+POOL_THREADS = 256  # rn_k_pool_reduce's block: thread t adds chains t, t + 256, ...
+
+
+def welford_restated(draws):
+    """the kernels' per-chain window statistics over draws [chains][L][n]: mean += od / k, raw += od * (q - mean), k the
+    position in the window, from mean = raw = 0.0.  Returns (mean, raw), each [chains][n]."""
+    draws = np.asarray(draws, dtype=np.float64)
+    mean, raw = np.zeros((draws.shape[0], draws.shape[2])), np.zeros((draws.shape[0], draws.shape[2]))
+    for k in range(draws.shape[1]):
+        q = draws[:, k]
+        od = q - mean
+        mean = mean + od / float(k + 1)
+        raw = raw + od * (q - mean)
+    return mean, raw
+
+
+def _block_sum(x):
+    """rn_k_pool_reduce's order over the chains of one rank, x [chains][n] -> [n]: thread t adds chains t, t + 256, ... left
+    to right starting from 0.0, then the halving tree red[t] += red[t + o], o = 128 ... 1"""
+    red = np.zeros((POOL_THREADS, x.shape[1]))
+    for j in range(0, x.shape[0], POOL_THREADS):
+        blk = x[j:j + POOL_THREADS]
+        red[:len(blk)] = red[:len(blk)] + blk
+    o = POOL_THREADS // 2
+    while o > 0:
+        red[:o] = red[:o] + red[o:2 * o]
+        o //= 2
+    return red[0]
+
+
+def pool_reduce_restated(mean, m2, L, ranks=1):
+    """rn_k_pool_reduce / rn_k_pool_apply in float64, in the kernels' order.  mean, m2: [chains][n] window statistics of
+    chains that each drew L positions; the chains are split over `ranks` as dist.chain_block splits them, and the two
+    all-reduces sum the ranks' buffers in rank order.  Returns (pool [2n+1] after the second all-reduce, variance [n],
+    the ranks' own buffers after pass 1 before it)."""
+    from rainier_b200 import dist
+
+    mean, m2 = np.asarray(mean, dtype=np.float64), np.asarray(m2, dtype=np.float64)
+    chains, n = mean.shape
+    blocks = [dist.chain_block(chains, r, ranks) for r in range(ranks)]
+    pools = []
+    for lo, hi in blocks:  # pass 0: pool[0] = chains, pool[1 + i] = sum of the means
+        p = np.zeros(2 * n + 1)
+        p[0], p[1:n + 1] = float(hi - lo), _block_sum(mean[lo:hi])
+        pools.append(p)
+    tot = pools[0][:n + 1].copy()
+    for p in pools[1:]:
+        tot = tot + p[:n + 1]
+    g = tot[1:] / tot[0]
+    for p, (lo, hi) in zip(pools, blocks):  # pass 1 around the pooled mean
+        p[:n + 1] = tot
+        d = mean[lo:hi] - g
+        p[n + 1:] = _block_sum(m2[lo:hi] + float(L) * d * d)
+    s = pools[0][n + 1:].copy()
+    for p in pools[1:]:
+        s = s + p[n + 1:]
+    pool = np.concatenate([tot, s])
+    return pool, s / (pool[0] * float(L)), [p.copy() for p in pools]
+
+
+def _dyadic(x):
+    """finite float64 values -> (Python ints a, e) with x[k] == a[k] * 2**e exactly"""
+    m, ex = np.frexp(np.asarray(x, dtype=np.float64).ravel())
+    mi, sh = (m * 2.0 ** 53).astype(np.int64).tolist(), (ex.astype(np.int64) - 53).tolist()
+    e = min(sh) if sh else 0
+    return [v << (s - e) for v, s in zip(mi, sh)], e
+
+
+def _scale(e):
+    return Fraction(2) ** e
+
+
+def pooled_variance_exact(draws):
+    """the population variance of all draws [chains][L][n] of a window, per parameter, in exact rational arithmetic around
+    the exact mean: (N sum q^2 - (sum q)^2) / N^2.  Returns a list of n Fractions."""
+    draws = np.asarray(draws, dtype=np.float64)
+    out = []
+    for i in range(draws.shape[2]):
+        a, e = _dyadic(draws[:, :, i])
+        N = len(a)
+        s1, s2 = sum(a), sum(v * v for v in a)
+        out.append(Fraction(N * s2 - s1 * s1, N * N) * _scale(2 * e))
+    return out
+
+
+def pooled_variance_exact_stats(mean, m2, L):
+    """the exact pooled population variance of C chains of L draws whose window means and M2 are exactly `mean`, `m2`
+    ([chains][n]): [sum_c M2_c + L sum_c (mean_c - g)^2] / (C L), g the exact mean of the means.  Returns n Fractions."""
+    mean, m2 = np.asarray(mean, dtype=np.float64), np.asarray(m2, dtype=np.float64)
+    chains = mean.shape[0]
+    out = []
+    for i in range(mean.shape[1]):
+        a, ea = _dyadic(mean[:, i])
+        b, eb = _dyadic(m2[:, i])
+        sa = sum(a)
+        between = Fraction(L * sum((chains * v - sa) ** 2 for v in a), chains * chains) * _scale(2 * ea)
+        out.append((Fraction(sum(b)) * _scale(eb) + between) / (chains * L))
+    return out
+
+
+def pool_error_bound(mean, m2, L, ranks=1, e_mean=0.0, e_m2=0.0):
+    """First-order bound on |var - var_exact|, per parameter: var = pool_reduce_restated(mean, m2, L, ranks)[1] (what the
+    kernels compute), var_exact the pooled population variance of draws whose exact per-chain window means and M2 lie
+    within e_mean, e_m2 ([chains][n] or scalars) of `mean`, `m2`.  Every floating-point operation rounds with relative
+    error at most u = 2^-53; products of two error terms are dropped (first order).
+      depth h = ceil(C_r / 256) + 8 + (R - 1): an addend passes through at most ceil(C_r / 256) additions in its thread,
+        the 8 levels of the 256-wide tree and R - 1 rank additions, so a computed sum of terms t_c errs by <= h u sum |t_c|;
+      pooled mean g = sum_c m_c / C:   |dg| <= mean_c(e_mean) + h u mean_c |m_c| + u |g|   (the division adds u |g|);
+      d_c = m_c - g:                   |dd_c| <= e_mean_c + |dg| + u |d_c|;
+      t_c = m2_c + (L d_c) d_c:        |dt_c| <= e_m2_c + 2 L |d_c| |dd_c| + 2 u L d_c^2 + u |t_c|   (two products, one sum);
+      var = sum_c t_c / (C L):         |dvar| <= (sum_c |dt_c| + h u sum_c |t_c|) / (C L) + u |var|
+    (C L is an integer below 2^53, so the product is exact).  Since sum_c M2_c + L sum_c (mu_c - g*)^2 is exactly C L times
+    the pooled variance for the exact chain means mu_c and their exact mean g*, this bounds the distance to var_exact."""
+    mean, m2 = np.asarray(mean, dtype=np.float64), np.asarray(m2, dtype=np.float64)
+    chains = mean.shape[0]
+    e_mean, e_m2 = np.broadcast_to(e_mean, mean.shape), np.broadcast_to(e_m2, mean.shape)
+    per_rank = -(-chains // ranks)
+    h = -(-per_rank // POOL_THREADS) + 8 + (ranks - 1)
+    pool, var, _ = pool_reduce_restated(mean, m2, L, ranks)
+    g = pool[1:mean.shape[1] + 1] / pool[0]
+    dg = e_mean.mean(axis=0) + h * U * np.abs(mean).mean(axis=0) + U * np.abs(g)
+    d = mean - g
+    dd = e_mean + dg + U * np.abs(d)
+    t = m2 + float(L) * d * d
+    dt = e_m2 + 2.0 * L * np.abs(d) * dd + 2.0 * U * L * d * d + U * np.abs(t)
+    return (dt.sum(axis=0) + h * U * np.abs(t).sum(axis=0)) / (chains * float(L)) + U * np.abs(var)
+
+
+def welford_error_bound(draws):
+    """First-order bounds (e_mean, e_m2), each [chains][n], on the distance between welford_restated(draws) (the kernels'
+    per-chain window statistics) and the exact mean / M2 of each chain's L draws.  Per chain and parameter let A = max |q|,
+    R = max q - min q, S = the computed M2, u = 2^-53.  The first update is exact (m_1 = q_1, its M2 term is q_1 * 0).
+      mean: m_k = m_(k-1) + (q_k - m_(k-1)) / k; the error of m_(k-1) is carried with weight 1 - 1/k <= 1, the update adds
+        u |q_k - m_(k-1)| / k (difference) + u |q_k - m_(k-1)| / k (division) + u |m_k| (sum), and |q_k - m_(k-1)| <= R,
+        |m_k| <= A, so |e_k| <= E = u (L A + 2 R H_L), H_L = 1 + 1/2 + ... + 1/L;
+      M2: sum_k (q_k - mean_(k-1)) (q_k - mean_k) is exactly S* for the exact running means; both factors are <= R and the
+        computed ones err by <= E + u R each, the product adds u R^2 and the running sum (non-decreasing, <= S) u S, so
+        |dS| <= L (2 R E + 3 u R^2 + u S)."""
+    draws = np.asarray(draws, dtype=np.float64)
+    L = draws.shape[1]
+    _, m2 = welford_restated(draws)
+    A, R = np.abs(draws).max(axis=1), draws.max(axis=1) - draws.min(axis=1)
+    E = U * (L * A + 2.0 * R * sum(1.0 / k for k in range(1, L + 1)))
+    return np.broadcast_to(E, m2.shape).copy(), L * (2.0 * R * E + 3.0 * U * R * R + U * np.abs(m2))
+
+
+def window_variance_bound(draws, ranks=1):
+    """first-order bound on |pooled window variance as the kernels compute it from draws [chains][L][n] - the exact one"""
+    mean, m2 = welford_restated(draws)
+    e_mean, e_m2 = welford_error_bound(draws)
+    return pool_error_bound(mean, m2, np.asarray(draws).shape[1], ranks, e_mean, e_m2)
+
+
+def textbook_variance(s1, s2, count):
+    """sum q^2 / N - mean^2 in float64 from pooled sums: the form that cancels when |mean| >> sd"""
+    mean = s1 / count
+    return s2 / count - mean * mean

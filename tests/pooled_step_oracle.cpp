@@ -1,11 +1,17 @@
-/* tests/pooled_step_oracle.cpp -- TEST INFRASTRUCTURE ONLY: the oracle's restatement of pooled step-size adaptation
- * (rn_config.step_adaptation == RN_ADAPT_POOLED, rainier_b200/csrc/rn_step_pool.cuh).  The reference adapts the step size
- * per chain; this extension shares one DualAvg over all chains, so the chains can no longer run one after another: a
- * lockstep driver runs iterations outer, chains inner, with the same exact integer sums as the kernels:
+/* tests/pooled_step_oracle.cpp -- TEST INFRASTRUCTURE ONLY: the oracle's restatement of the two pooled adaptation modes,
+ * pooled step sizes (rn_config.step_adaptation == RN_ADAPT_POOLED, rainier_b200/csrc/rn_step_pool.cuh) and pooled mass
+ * windows (rn_config.adaptation == RN_ADAPT_POOLED, rn_k_pool_reduce / rn_k_pool_apply).  The reference adapts per chain;
+ * these extensions share state over all chains, so the chains can no longer run one after another: a lockstep driver runs
+ * iterations outer, chains inner.
+ * Pooled steps, with the same exact integer sums as the kernels:
  *   1. k_c = log2 of chain c's findReasonableStepSize (clamped to [-1075, 1024]); eps0 = jexp(ln2 * (K / C))
  *   2. q_c = rint(jexp(a_c) * 2^32), P_t = Q_t / (2^32 C), DualAvg.update with newAcceptanceProb = P_t
- *   3. Driver.scala:67-80 order: step update, mass update, stepSizeTuner.reset() when a window closed
- *   4. sampling at jexp(logStepSizeBar); Stats stay per chain
+ * Pooled mass windows (diagonal tuner), in rn_k_pool_reduce's summation order:
+ *   per chain, Welford statistics of the window: mean += od / win_i, raw += od * (q - mean) (win_i: position in the window)
+ *   at the window end, pass 0: 256 partials (thread t adds chains t, t + 256, ... from 0.0), halving tree, / C = pooled mean;
+ *   pass 1: the same over raw_c + L (mean_c - pooled mean)^2; variance = sum / (C L); error flag 2 where !(variance > 0)
+ * Both: Driver.scala:67-80 order (step update, mass update, stepSizeTuner.reset() when a window closed), sampling at the
+ * final step size; Stats stay per chain.
  * The per-chain oracle (oracle/rainier_oracle.cpp) is compiled into this library unchanged and only extended. */
 #include "../oracle/rainier_oracle.cpp"
 
@@ -18,7 +24,10 @@ struct LockstepChain {
   std::unique_ptr<LeapFrog> lf;
   std::unique_ptr<Sampler> sampler;
   std::unique_ptr<MassMatrixTuner> massTuner;
+  std::unique_ptr<StepSizeTuner> stepTuner;  /* per-chain steps only */
+  double stepSize = 0.0;
   std::vector<double> params;
+  std::vector<double> wmean, wraw;           /* pooled mass windows: the chain's Welford statistics of the window */
   MassMatrix mass;
   RNG rng;
   ChainResult res;
@@ -27,12 +36,45 @@ struct LockstepChain {
 static const double kLn2 = 0.6931471805599453;
 static const double kQScale = 4294967296.0;
 
-/* trace: optional [chains][warmup+iterations][4], as driver_sample writes it */
+/* rn_k_pool_reduce restated (one rank): the pooled population variance of the window that just closed, L draws per chain */
+static void pool_reduce(const std::vector<LockstepChain>& ch, int n, int L, std::vector<double>& var) {
+  const int C = (int)ch.size();
+  std::vector<double> pool(2 * (size_t)n + 1, 0.0);
+  double red[256];
+  for (int pass = 0; pass < 2; pass++)
+    for (int i = 0; i < n; i++) {
+      const double gmean = pass ? pool[1 + i] / pool[0] : 0.0;
+      for (int t = 0; t < 256; t++) {
+        double acc = 0.0;
+        for (int c = t; c < C; c += 256) {
+          if (pass) {
+            const double d = ch[c].wmean[i] - gmean;
+            acc += ch[c].wraw[i] + (double)L * d * d;
+          } else {
+            acc += ch[c].wmean[i];
+          }
+        }
+        red[t] = acc;
+      }
+      for (int o = 128; o > 0; o >>= 1)
+        for (int t = 0; t < o; t++) red[t] += red[t + o];
+      pool[1 + (pass ? n : 0) + i] = red[0];
+      if (!pass && i == 0) pool[0] = (double)C;
+    }
+  for (int i = 0; i < n; i++) var[i] = pool[1 + n + i] / (pool[0] * (double)L);
+}
+
+/* trace: optional [chains][warmup+iterations][4], as driver_sample writes it; warm: optional [chains][warmup][n], the
+ * position after every warmup iteration (what the mass-matrix tuner sees); win_mass: optional [windows][n], the pooled
+ * variance of every window that closed */
 static void lockstep_sample(const Model& model, const rn_config& cfg, std::vector<RNG>& rngs, double* samples, double* mass_out,
-                            size_t mass_stride, rn_chain_stats* stats, double* trace, int& error_flags) {
+                            size_t mass_stride, rn_chain_stats* stats, double* trace, double* warm, double* win_mass,
+                            int& error_flags) {
   const int C = (int)rngs.size();
   const int n = model.n();
   const size_t T = (size_t)cfg.warmup_iterations + (size_t)cfg.iterations;
+  const bool pooled_step = cfg.step_adaptation == RN_ADAPT_POOLED;
+  const bool pooled_mass = cfg.adaptation == RN_ADAPT_POOLED && cfg.mass_tuner == RN_MASS_DIAGONAL;
   std::vector<LockstepChain> ch(C);
   DualAvgTuner finder(cfg.delta);
   int64_t K = 0;
@@ -50,6 +92,14 @@ static void lockstep_sample(const Model& model, const rn_config& cfg, std::vecto
     MassMatrix identity;
     x.params = x.lf->initialize(identity, x.rng);     /* Driver.scala:22 */
     x.sampler->initialize(x.params, *x.lf, x.rng);    /* :59 */
+    x.wmean.assign(n, 0.0);
+    x.wraw.assign(n, 0.0);
+    if (!pooled_step) { /* :60, per chain */
+      x.stepTuner = make_step_tuner(cfg);
+      x.stepSize = x.stepTuner->initialize(x.params, *x.lf);
+      x.mass = x.massTuner->initialize(*x.lf, cfg.warmup_iterations); /* :61 */
+      continue;
+    }
     const double s0 = finder.findReasonableStepSize(x.params, *x.lf, identity);
     int k;                                            /* s0 == 2^k exactly (0 = 2^-1075, inf = 2^1024) */
     if (s0 == 0.0)
@@ -63,9 +113,10 @@ static void lockstep_sample(const Model& model, const rn_config& cfg, std::vecto
     K += std::max(-1075, std::min(1024, k));
     x.mass = x.massTuner->initialize(*x.lf, cfg.warmup_iterations); /* :61 */
   }
-  double stepSize = jexp(kLn2 * ((double)K / (double)C)); /* eps0: what DualAvgTuner.initialize returns (DualAvg.scala:6-10) */
+  double stepSize = pooled_step ? jexp(kLn2 * ((double)K / (double)C)) : 0.0; /* eps0: what DualAvgTuner.initialize returns (DualAvg.scala:6-10) */
   DualAvg da = DualAvg::apply(cfg.delta, stepSize);
-  std::vector<double> sample(n);
+  std::vector<double> sample(n), var(n);
+  int win_size = cfg.initial_window_size, win_i = 0, win_j = 0, windows = 0; /* pooled mass windows: the same for every chain */
   for (int t = 0; t < cfg.warmup_iterations; t++) { /* Driver.scala:67-88, chains in lockstep */
     int64_t Q = 0;
     bool closed = false;
@@ -73,17 +124,21 @@ static void lockstep_sample(const Model& model, const rn_config& cfg, std::vecto
       LockstepChain& x = ch[c];
       const int64_t steps0 = x.lf->stats.leapfrogSteps;
       const int acc0 = x.lf->stats.accepted;
-      const double a = x.sampler->warmup(x.params, *x.lf, stepSize, x.mass, x.rng);
-      Q += (int64_t)std::rint(jexp(a) * kQScale);
+      const double used = pooled_step ? stepSize : x.stepSize;
+      const double a = x.sampler->warmup(x.params, *x.lf, used, x.mass, x.rng);
+      if (pooled_step)
+        Q += (int64_t)std::rint(jexp(a) * kQScale);
+      else
+        x.stepSize = x.stepTuner->update(a); /* :69 */
       if (trace) {
         double* tr = trace + ((size_t)c * T + (size_t)t) * 4;
         tr[0] = a;
         tr[1] = (double)(x.lf->stats.accepted - acc0);
-        tr[2] = stepSize;
+        tr[2] = used;
         tr[3] = (double)(x.lf->stats.leapfrogSteps - steps0);
       }
     }
-    { /* stepSizeTuner.update(P_t), DualAvg.scala:58-77 */
+    if (pooled_step) { /* stepSizeTuner.update(P_t), DualAvg.scala:58-77 */
       const double newAcceptanceProb = (double)Q / (kQScale * (double)C);
       da.iteration = da.iteration + 1;
       double avgErrorMultiplier = 1.0 / ((double)da.iteration + da.acceptanceProbUpdateDenom);
@@ -93,26 +148,67 @@ static void lockstep_sample(const Model& model, const rn_config& cfg, std::vecto
       da.logStepSizeBar = (stepSizeMultiplier * da.logStepSize + (1.0 - stepSizeMultiplier) * da.logStepSizeBar);
       stepSize = da.stepSize();
     }
-    for (int c = 0; c < C; c++) { /* massMatrixTuner.update, :74-80 (the windows close on the same iteration for every chain) */
-      LockstepChain& x = ch[c];
-      x.lf->variables(x.params, sample.data());
-      MassMatrix m;
-      if (x.massTuner->update(sample.data(), m)) {
-        x.mass = m;
-        if (m.invalid) x.res.error_flags |= 2;
+    if (pooled_mass) { /* massMatrixTuner.update, :74-80, with the window statistics pooled over all chains */
+      win_j += 1;
+      const bool in_window = !(win_j < cfg.skip_first || (cfg.warmup_iterations - win_j) < cfg.skip_last);
+      if (in_window) win_i += 1;
+      for (int c = 0; c < C; c++) {
+        LockstepChain& x = ch[c];
+        x.lf->variables(x.params, sample.data());
+        if (warm) std::memcpy(warm + ((size_t)c * cfg.warmup_iterations + t) * n, sample.data(), sizeof(double) * n);
+        if (!in_window) continue;
+        for (int i = 0; i < n; i++) {
+          double mean = x.wmean[i];
+          const double od = sample[i] - mean;
+          mean += od / (double)win_i;
+          x.wmean[i] = mean;
+          x.wraw[i] += od * (sample[i] - mean);
+        }
+      }
+      if (in_window && win_i == win_size) {
+        pool_reduce(ch, n, win_size, var);
+        if (win_mass) std::memcpy(win_mass + (size_t)windows * n, var.data(), sizeof(double) * n);
+        windows += 1;
+        win_i = 0;
+        win_size = jd2i(win_size * cfg.window_expansion);
         closed = true;
+        for (int c = 0; c < C; c++) {
+          LockstepChain& x = ch[c];
+          x.mass = DiagonalMassMatrix(var);
+          for (int i = 0; i < n; i++) {
+            if (!(var[i] > 0.0)) x.res.error_flags |= 2;
+            x.wmean[i] = 0.0;
+            x.wraw[i] = 0.0;
+          }
+        }
+      }
+    } else {
+      for (int c = 0; c < C; c++) { /* massMatrixTuner.update, :74-80 (the windows close on the same iteration for every chain) */
+        LockstepChain& x = ch[c];
+        x.lf->variables(x.params, sample.data());
+        if (warm) std::memcpy(warm + ((size_t)c * cfg.warmup_iterations + t) * n, sample.data(), sizeof(double) * n);
+        MassMatrix m;
+        if (x.massTuner->update(sample.data(), m)) {
+          x.mass = m;
+          if (m.invalid) x.res.error_flags |= 2;
+          closed = true;
+        }
       }
     }
     if (closed) { /* stepSizeTuner.reset(), DualAvg.scala:17-21 */
-      const double ss = da.finalStepSize();
-      da = DualAvg::apply(cfg.delta, ss);
-      stepSize = ss;
+      if (pooled_step) {
+        const double ss = da.finalStepSize();
+        da = DualAvg::apply(cfg.delta, ss);
+        stepSize = ss;
+      } else {
+        for (LockstepChain& x : ch) x.stepSize = x.stepTuner->reset();
+      }
     }
   }
-  const double finalStep = da.finalStepSize(); /* Driver.scala:37 */
   for (int c = 0; c < C; c++) {
     LockstepChain& x = ch[c];
     LeapFrog& lf = *x.lf;
+    const double finalStep = pooled_step ? da.finalStepSize() : x.stepTuner->stepSize(); /* Driver.scala:37 */
     lf.resetStats(); /* :31 */
     for (int i = 0; i < cfg.iterations; i++) {
       const int64_t steps0 = lf.stats.leapfrogSteps;
@@ -171,11 +267,15 @@ static void lockstep_sample(const Model& model, const rn_config& cfg, std::vecto
 } /* namespace rno */
 
 extern "C" {
-/* rno_sample_traced for cfg->step_adaptation == RN_ADAPT_POOLED (pooled mass windows are not restated here) */
+/* rno_sample_traced for pooled step sizes (cfg->step_adaptation == RN_ADAPT_POOLED, DualAvg) and / or pooled diagonal mass
+ * windows (cfg->adaptation == RN_ADAPT_POOLED); warm: optional [chains][warmup][n] warmup positions; win_mass: optional
+ * [windows][n] pooled variance of every closed window */
 int rno_sample_pooled_step(rno_model* mm, const rn_config* cfg, const int64_t* seeds, int chains, double* samples, double* mass,
-                           rn_chain_stats* stats, double* trace) {
-  if (cfg->step_adaptation != RN_ADAPT_POOLED || cfg->step_size_tuner != RN_STEP_DUAL_AVG || cfg->adaptation != RN_ADAPT_PER_CHAIN)
-    return fail(RN_E_UNSUPPORTED, "the lockstep oracle covers pooled DualAvg steps with per-chain mass windows");
+                           rn_chain_stats* stats, double* trace, double* warm, double* win_mass) {
+  const bool pooled_step = cfg->step_adaptation == RN_ADAPT_POOLED, pooled_mass = cfg->adaptation == RN_ADAPT_POOLED;
+  if ((pooled_step && cfg->step_size_tuner != RN_STEP_DUAL_AVG) || (pooled_mass && cfg->mass_tuner != RN_MASS_DIAGONAL) ||
+      !(pooled_step || pooled_mass))
+    return fail(RN_E_UNSUPPORTED, "the lockstep oracle covers pooled DualAvg steps and pooled diagonal mass windows");
   const Model& m = mm->m;
   const int n = m.n();
   const size_t mass_stride = (cfg->mass_tuner == RN_MASS_DENSE || (cfg->mass_tuner == RN_MASS_STATIC && cfg->static_matrix == RN_MATRIX_DENSE))
@@ -184,7 +284,7 @@ int rno_sample_pooled_step(rno_model* mm, const rn_config* cfg, const int64_t* s
   std::vector<RNG> rngs(chains);
   for (int c = 0; c < chains; c++) rngs[c].rand = JRandom(seeds[c]); /* ScalaRNG(seed), S/RNG.scala:20-26 */
   int err = 0;
-  lockstep_sample(m, *cfg, rngs, samples, mass, mass_stride, stats, trace, err);
+  lockstep_sample(m, *cfg, rngs, samples, mass, mass_stride, stats, trace, warm, win_mass, err);
   if (err & 1) return fail(RN_E_LOOKUP, "lookup index out of range");
   if (err & 2) return fail(RN_E_INVALID, "requirement failed: adapted mass matrix contains 0.0 (MassMatrix.scala:8,16)");
   return RN_OK;
