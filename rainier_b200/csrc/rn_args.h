@@ -1,5 +1,5 @@
 // rn_args.h -- kernel argument block shared verbatim by the host runtime (rn_runtime.cpp) and the device code
-// (embedded in front of rn_sampler.cuh).  Plain C: only int / long long / double / pointers.
+// (embedded in front of rn_sampler_common.cuh).  Plain C: only int / long long / double / pointers.
 #ifndef RN_ARGS_H
 #define RN_ARGS_H
 #ifndef RN_PRELUDE_CUH
@@ -54,7 +54,7 @@ struct RnArgs {
   int chain_begin;               // rn_k_iter works on chains [chain_begin, chain_end): rn_sample pipelines chain blocks
   int chain_end;                 //   against the device->host copy of the previous block
   int pad1;
-  // pooled step-size adaptation (RN_STEP_POOL modules only, rn_step_pool.cuh): rn_k_init adds into step_acc[0] (sum of
+  // pooled step-size adaptation (RN_STEP_POOL modules only, rn_sampler_common.cuh): rn_k_init adds into step_acc[0] (sum of
   // the chains' log2 initial step sizes) and step_acc[1] (chains); a warmup launch of one iteration adds its quantised
   // acceptance probabilities into *step_acc (the slot of that iteration)
   rn_i64* step_acc;

@@ -14,10 +14,9 @@
 namespace rn {
 
 extern const char* kPreludeSource;  // rn_prelude.cuh, embedded at build time
-extern const char* kSamplerSource;     // rn_args.h + rn_sampler.cuh
-extern const char* kSamplerWpcSource;  // rn_args.h + rn_sampler_wpc.cuh
-extern const char* kStepPoolSource;       // rn_step_pool.cuh (RN_STEP_POOL modules)
-extern const char* kStepPoolApplySource;  // rn_step_pool_apply.cuh (RN_STEP_POOL modules)
+extern const char* kSamplerCommonSource;  // rn_args.h + rn_sampler_common.cuh
+extern const char* kSamplerSource;        // rn_sampler.cuh + rn_diag.cuh
+extern const char* kSamplerWpcSource;     // rn_sampler_wpc.cuh + rn_diag.cuh
 extern const char* kFunctionSource;    // rn_function.cuh
 extern const char* kOptimizerSource;   // rn_args.h + rn_optimizer.cuh
 
@@ -1887,8 +1886,7 @@ std::string emit_source(const Program& P, const EmitOptions& opt) {
       os << "#define RN_TMA_TILE_DOUBLES " << ((opt.mma && z.mma_ok) ? z.mma_shared_doubles : z.tile_doubles) << "\n";
     }
   }
-  os << kPreludeSource << "\n";
-  if (opt.step_pool) os << kStepPoolSource << "\n";
+  os << kPreludeSource << "\n" << kSamplerCommonSource << "\n";
   if (opt.backend == 1)  // (RN_WPC_SCRATCH is defined by the emitted density; macros expand where they are used)
     os << "#define RN_WPC_SMEM_DOUBLES (" << wpc_vectors(opt) << " * RN_N + RN_WPC_SCRATCH)\n";
   os << emit_density(P, opt) << "\n";
@@ -1897,7 +1895,6 @@ std::string emit_source(const Program& P, const EmitOptions& opt) {
   } else {
     os << kSamplerSource << "\n";
   }
-  if (opt.step_pool) os << kStepPoolApplySource << "\n";
   return os.str();
 }
 

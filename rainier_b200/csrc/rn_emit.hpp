@@ -13,7 +13,7 @@ struct EmitOptions {
   bool fast_math = false; // strength-reduce constant powers beyond what Math.pow itself special-cases
   int mass_max = 0;       // 0 identity only, 1 + diagonal, 2 + dense
   bool enable_ehmc = false;
-  bool step_pool = false; // pooled step-size adaptation (rn_step_pool.cuh): RN_STEP_POOL kernels
+  bool step_pool = false; // pooled step-size adaptation (rn_sampler_common.cuh): RN_STEP_POOL kernels
   int tma_stages = 0;     // warp per chain: shared-memory stages of the CTA-shared data-tile pipeline (0 = off)
   int wpc_k = 1;          // warp per chain: warps owning one chain (1, 2, 4 or 8; > 1 for chains with a large state)
   std::vector<uint64_t> target_base;  // per target: element offset of its tile-major [tile][column][pitch] block in the data buffer

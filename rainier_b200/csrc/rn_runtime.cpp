@@ -1003,7 +1003,7 @@ struct rn_sampler {
   size_t trace_iters = 0, trace_pos = 0;
   rn_comm* comm = nullptr;
   CUdeviceptr d_pool = 0;  // [2n+1] pooled window statistics (RN_ADAPT_POOLED)
-  CUdeviceptr d_step = 0;  // int64 [2 + warmup]: K, C, Q_t of pooled step-size adaptation (rn_step_pool.cuh), zeroed at create
+  CUdeviceptr d_step = 0;  // int64 [2 + warmup]: K, C, Q_t of pooled step-size adaptation (rn_sampler_common.cuh), zeroed at create
   // device time of the sampling phase (Stats.gradientTimes / iterationTimes, Stats.scala:8-9): events bracket every
   // batch of phase-1 launches; closed spans are summed when the stats are read
   CUevent ev_run[2] = {nullptr, nullptr};
@@ -1356,7 +1356,7 @@ static int pool_window(const Api* A, rn_sampler* s, int window_len) {
   return RN_OK;
 }
 
-// pooled step-size adaptation (rn_step_pool.cuh): all-reduce the int64 sums of slot `slot` (.. + count) over the ranks, then
+// pooled step-size adaptation (rn_sampler_common.cuh): all-reduce the int64 sums of slot `slot` (.. + count) over the ranks, then
 // rn_k_step_pool(t, reset) on every chain
 static int step_pool_apply(const Api* A, rn_sampler* s, int slot, int count, int t, int reset) {
   int rc = comm_allreduce(A, s, s->d_step + (size_t)slot * 8, (size_t)count, 4 /*ncclInt64*/);

@@ -20,13 +20,7 @@
 #ifndef RN_SAMPLER_CUH
 #define RN_SAMPLER_CUH
 
-// struct RnArgs: see rn_args.h (shared verbatim with the host runtime)
-
-#define RN_LN2 0.6931471805599453
-#ifndef RN_STEP_POOL
-#define RN_STEP_POOL 0 /* 1: pooled step-size adaptation (rn_step_pool.cuh, rn_step_pool_apply.cuh) */
-#endif
-#define RN_AT(ptr, field, c) (ptr)[(size_t)(field) * (size_t)A.chains + (size_t)(c)]
+// struct RnArgs: see rn_args.h (shared verbatim with the host runtime); RN_AT and the adaptation arithmetic: rn_sampler_common.cuh
 
 // ---- this thread's COLD state lives in shared memory -----------------------------------------------------------
 // Everything a chain touches once per iteration is kept out of registers: the Stats counters, the RNG state, the energies
@@ -477,7 +471,7 @@ RN_GLOBAL void rn_k_init(const RnArgs A) {
     const double exponent = (lap > -RN_LN2) ? 1.0 : -1.0;
     const double doubleOrHalf = (exponent > 0) ? 2.0 : 0.5;
 #if RN_STEP_POOL
-    int log2Step = 0;  // stepSize == 2^log2Step (doubling / halving 1.0 is exact down to 0 = 2^-1075 and up to inf = 2^1024)
+    int log2Step = 0;  // stepSize == 2^log2Step
 #endif
     while (stepSize != 0.0 && (exponent * lap > -exponent * RN_LN2)) {
       stepSize *= doubleOrHalf;
@@ -494,16 +488,10 @@ RN_GLOBAL void rn_k_init(const RnArgs A) {
       rn_leapfrog(A, c, T, 0, s, 1, stepSize, S);
       lap = rn_log_accept(rn_energy(A, c, T, s, 0, s.U) - H0);
     }
-    // DualAvg.apply, DualAvg.scala:80-90
-    RN_AT(A.da, 1, c) = rn_log(stepSize);
-    RN_AT(A.da, 2, c) = 0.0;
-    RN_AT(A.da, 3, c) = 0.0;
-    RN_AT(A.da, 4, c) = rn_log(10 * stepSize);
-    A.da_iter[c] = 0;
+    rn_da_apply(stepSize, RN_AT(A.da, 1, c), RN_AT(A.da, 2, c), RN_AT(A.da, 3, c), RN_AT(A.da, 4, c), A.da_iter[c]);
 #if RN_STEP_POOL
     // pooled: K and C over all chains; rn_k_step_pool replaces this chain's DualAvg with the shared one
-    rn_pool_add(A.step_acc + 0, log2Step < -1075 ? -1075 : (log2Step > 1024 ? 1024 : log2Step));
-    rn_pool_add(A.step_acc + 1, 1);
+    rn_pool_add_initial_step(A.step_acc, log2Step);
 #endif
   } else {
     stepSize = A.static_step;
@@ -744,6 +732,8 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
       // pooled: this chain's share of the iteration's acceptance sum; rn_k_step_pool applies the update (and any reset)
       if (A.step_tuner == 0) rn_pool_add(A.step_acc + it, rn_pool_quantise(rn_exp(a)));
 #else
+      // Written out rather than rn_da_update: through the helper, fast-math builds of this kernel contract the update's
+      // products into FMAs differently, which changes the adapted step sizes (parity builds are unaffected).
       if (A.step_tuner == 0) {
         const double newAcceptanceProb = rn_exp(a);
         const int daIter = A.da_iter[c] + 1;
@@ -765,40 +755,32 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
         if (A.adaptation == 1) {
           // pooled extension: per-chain Welford statistics of the window; combined over chains (and ranks) at the window
           // end (rn_k_pool_reduce / rn_k_pool_apply) -- launches are cut at window ends in this mode
-          if (!(win_j < A.skip_first || (A.total_warmup - win_j) < A.skip_last)) {
+          if (RN_IN_WINDOW(A, win_j)) {
             win_i += 1;
             RN_UNROLL
             for (int i = 0; i < RN_N; i++) {  // the chain's Welford mean / M2 over this window
-              double mean = RN_AT(A.est_mean, i, c);
-              const double od = s.q[i] - mean;
-              mean += od / (double)win_i;
-              RN_AT(A.est_mean, i, c) = mean;
-              RN_AT(A.est_raw, i, c) += od * (s.q[i] - mean);
+              double oldDiff;
+              rn_variance_update(A, c, i, s.q[i], win_i, oldDiff);
             }
             if (win_i == win_size) {
               win_i = 0;
               win_size = rn_d2i(win_size * A.win_expansion);
             }
           }
-        } else if (!(win_j < A.skip_first || (A.total_warmup - win_j) < A.skip_last)) {
+        } else if (RN_IN_WINDOW(A, win_j)) {
           win_i += 1;
-          est_samples += 1;  // VarianceEstimator.update, MassMatrixEstimator.scala:69-83
+          est_samples += 1;
 #if RN_MASS_MAX >= 2
           double oldDiff[RN_N], newDiff[RN_N];
-#endif
+          RN_UNROLL
+          for (int i = 0; i < RN_N; i++) newDiff[i] = rn_variance_update(A, c, i, s.q[i], est_samples, oldDiff[i]);
+#else
           RN_UNROLL
           for (int i = 0; i < RN_N; i++) {
-            double mean = RN_AT(A.est_mean, i, c);
-            const double od = s.q[i] - mean;
-            mean += (od / (double)est_samples);
-            const double nd = s.q[i] - mean;
-            RN_AT(A.est_mean, i, c) = mean;
-            RN_AT(A.est_raw, i, c) += od * nd;
-#if RN_MASS_MAX >= 2
-            oldDiff[i] = od;
-            newDiff[i] = nd;
-#endif
+            double oldDiff;
+            rn_variance_update(A, c, i, s.q[i], est_samples, oldDiff);
           }
+#endif
 #if RN_MASS_MAX >= 2
           if (A.mass_tuner == 2) {  // CovarianceEstimator.update, :28-41
             for (int j = 0; j < RN_N; j++)
@@ -836,39 +818,13 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
                 RN_AT(A.est_raw, i, c) = 0.0;
               }
               double lower[(RN_N * (RN_N + 1)) / 2];
-              int l = 0;
-              for (int i = 0; i < RN_N; i++)
-                for (int k = 0; k <= i; k++) {
-                  double sum = 0.0;
-                  for (int j = 0; j < k; j++) sum += lower[(i * (i + 1)) / 2 + j] * lower[(k * (k + 1)) / 2 + j];
-                  const double x = RN_AT(A.mass, i * RN_N + k, c) - sum;
-                  if (i == k)
-                    lower[l] = sqrt(x);
-                  else {
-                    const double diag = lower[((k + 1) * (k + 2)) / 2 - 1];
-                    lower[l] = (1.0 / diag * x);
-                  }
-                  l += 1;
-                }
-              l = 0;
-              for (int i = 0; i < RN_N; i++)
-                for (int k = 0; k < (RN_N - i); k++) {
-                  RN_AT(A.chol, l, c) = lower[((k + i) * (k + i + 1)) / 2 + i];
-                  l += 1;
-                }
+              rn_cholesky_upper(A, c, lower, 1);
             }
 #endif
             // stepSize = stepSizeTuner.reset(), Driver.scala:78 / DualAvg.scala:17-21 (pooled steps: rn_k_step_pool)
 #if !RN_STEP_POOL
-            if (A.step_tuner == 0) {
-              const double ss = rn_exp(RN_AT(A.da, 2, c));
-              RN_AT(A.da, 1, c) = rn_log(ss);
-              RN_AT(A.da, 2, c) = 0.0;
-              RN_AT(A.da, 3, c) = 0.0;
-              A.da_iter[c] = 0;
-              RN_AT(A.da, 4, c) = rn_log(10 * ss);
-              stepSize = ss;
-            }
+            if (A.step_tuner == 0)
+              stepSize = rn_da_reset(RN_AT(A.da, 1, c), RN_AT(A.da, 2, c), RN_AT(A.da, 3, c), RN_AT(A.da, 4, c), A.da_iter[c]);
 #endif
           }
         }
@@ -922,89 +878,5 @@ RN_GLOBAL void rn_k_density(const double* RN_RESTRICT qin, double* RN_RESTRICT o
   if (e) atomicOr(err, e);
 #endif
 }
-
-// =============================================================================================================
-// rn_k_transpose: [rows][cols] -> [cols][rows] (sample chunks [iter][n][chain] -> [chain][iter][n] before the
-// device->host copy of rn_sample).  32x32 tiles through shared memory, both sides coalesced.
-// =============================================================================================================
-#ifndef RN_HOST_EMULATION
-RN_GLOBAL void rn_k_transpose(const double* RN_RESTRICT src, double* RN_RESTRICT dst, int rows, int cols,
-                              long long src_ld, long long dst_ld, long long dst_off) {
-  // dst[c * dst_ld + dst_off + r] = src[r * src_ld + c]   (a block of `cols` chains out of src_ld)
-  __shared__ double tile[32][33];
-  const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
-  for (int j = threadIdx.y; j < 32; j += 8) {
-    const int r = r0 + j, c = c0 + threadIdx.x;
-    if (r < rows && c < cols) tile[j][threadIdx.x] = src[(size_t)r * (size_t)src_ld + c];
-  }
-  __syncthreads();
-  for (int j = threadIdx.y; j < 32; j += 8) {
-    const int c = c0 + j, r = r0 + threadIdx.x;
-    if (r < rows && c < cols) dst[(size_t)c * (size_t)dst_ld + (size_t)dst_off + r] = tile[threadIdx.x][j];
-  }
-}
-#endif
-
-// =============================================================================================================
-// Pooled mass-matrix adaptation (RN_ADAPT_POOLED; an extension, not reference semantics): at a window end the chains'
-// Welford statistics of the window (mean_c, M2_c over L draws) are combined over all chains of this GPU and, through two
-// small ncclAllReduce calls, over all ranks: first the means (-> pooled mean), then M2_c + L (mean_c - mean)^2 (Chan's
-// parallel variance: no s2/n - mean^2 cancellation).  Reductions run in a fixed order (no atomics): the shared diagonal
-// mass matrix is reproducible run to run.  It is applied to every chain, statistics cleared, DualAvg restarted from each
-// chain's averaged step size (Driver.scala:75-80).
-// =============================================================================================================
-#ifndef RN_HOST_EMULATION
-RN_GLOBAL void rn_k_pool_reduce(const RnArgs A, double* pool, int window_len, int pass) {
-  // One block per parameter; thread t adds chains t, t + 256, ... in order, then a fixed tree: the result does not depend
-  // on scheduling (no atomics).  pass 0: pool[1 + i] = sum over chains of the chain's window mean, pool[0] = chains.
-  // pass 1 (after the all-reduce of pass 0): pool[1 + n + i] = sum over chains of [M2_c + L (mean_c - mean)^2] -- Chan's
-  // combination of the chains' Welford statistics around the POOLED mean (no s2/n - mean^2 cancellation).
-  __shared__ double red[256];
-  const int i = (int)blockIdx.x;
-  const double gmean = pass ? pool[1 + i] / pool[0] : 0.0;
-  const double* mean = A.est_mean + (size_t)i * A.chains;
-  const double* m2 = A.est_raw + (size_t)i * A.chains;
-  double acc = 0.0;
-  for (int c = (int)threadIdx.x; c < A.chains; c += (int)blockDim.x) {
-    if (pass) {
-      const double d = mean[c] - gmean;
-      acc += m2[c] + (double)window_len * d * d;
-    } else {
-      acc += mean[c];
-    }
-  }
-  red[threadIdx.x] = acc;
-  __syncthreads();
-  for (int o = (int)blockDim.x / 2; o > 0; o >>= 1) {
-    if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    pool[1 + (pass ? RN_N : 0) + i] = red[0];
-    if (!pass && i == 0) pool[0] = (double)A.chains;
-  }
-}
-RN_GLOBAL void rn_k_pool_apply(const RnArgs A, const double* pool, int window_len) {
-  const int c = (int)(blockIdx.x * blockDim.x + threadIdx.x);
-  if (c >= A.chains) return;
-  const double cnt = pool[0] * (double)window_len;  // draws of the window over all chains of all ranks
-  for (int i = 0; i < RN_N; i++) {
-    const double var = pool[1 + RN_N + i] / cnt;
-    if (!(var > 0.0)) A.st_err[c] |= 2;
-    RN_AT(A.mass, i, c) = var;
-    RN_AT(A.est_mean, i, c) = 0.0;
-    RN_AT(A.est_raw, i, c) = 0.0;
-  }
-  if (A.step_tuner == 0) {  // stepSizeTuner.reset(), DualAvg.scala:17-21
-    const double ss = rn_exp(RN_AT(A.da, 2, c));
-    RN_AT(A.da, 0, c) = ss;
-    RN_AT(A.da, 1, c) = rn_log(ss);
-    RN_AT(A.da, 2, c) = 0.0;
-    RN_AT(A.da, 3, c) = 0.0;
-    RN_AT(A.da, 4, c) = rn_log(10 * ss);
-    A.da_iter[c] = 0;
-  }
-}
-#endif
 
 #endif  // RN_SAMPLER_CUH

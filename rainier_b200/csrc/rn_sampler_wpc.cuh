@@ -20,11 +20,7 @@
 #ifndef RN_SAMPLER_WPC_CUH
 #define RN_SAMPLER_WPC_CUH
 
-#define RN_LN2 0.6931471805599453
-#ifndef RN_STEP_POOL
-#define RN_STEP_POOL 0 /* 1: pooled step-size adaptation (rn_step_pool.cuh, rn_step_pool_apply.cuh) */
-#endif
-#define RN_AT(ptr, field, c) (ptr)[(size_t)(field) * (size_t)A.chains + (size_t)(c)]
+// RnArgs (rn_args.h), RN_AT and the adaptation arithmetic: rn_sampler_common.cuh
 #define RN_LANE ((int)(threadIdx.x % RN_G))  // thread index inside the chain's group (RN_G, RN_SYNC: rn_prelude.cuh)
 #define RN_FOR_LANES(i) for (int i = RN_LANE; i < RN_N; i += RN_G)
 
@@ -313,7 +309,7 @@ RN_GLOBAL void rn_k_init(const RnArgs A) {
     const double exponent = (lap > -RN_LN2) ? 1.0 : -1.0;
     const double doubleOrHalf = (exponent > 0) ? 2.0 : 0.5;
 #if RN_STEP_POOL
-    int log2Step = 0;  // stepSize == 2^log2Step (see rn_sampler.cuh)
+    int log2Step = 0;  // stepSize == 2^log2Step
 #endif
     while (stepSize != 0.0 && (exponent * lap > -exponent * RN_LN2)) {
       stepSize *= doubleOrHalf;
@@ -332,15 +328,10 @@ RN_GLOBAL void rn_k_init(const RnArgs A) {
       lap = rn_log_accept(rn_energy(w, w.p, w.U) - H0);
     }
     if (RN_LANE == 0) {
-      RN_AT(A.da, 1, c) = rn_log(stepSize);
-      RN_AT(A.da, 2, c) = 0.0;
-      RN_AT(A.da, 3, c) = 0.0;
-      RN_AT(A.da, 4, c) = rn_log(10 * stepSize);
-      A.da_iter[c] = 0;
+      rn_da_apply(stepSize, RN_AT(A.da, 1, c), RN_AT(A.da, 2, c), RN_AT(A.da, 3, c), RN_AT(A.da, 4, c), A.da_iter[c]);
 #if RN_STEP_POOL
       // pooled: K and C over all chains, one lane per chain; rn_k_step_pool installs the shared DualAvg
-      rn_pool_add(A.step_acc + 0, log2Step < -1075 ? -1075 : (log2Step > 1024 ? 1024 : log2Step));
-      rn_pool_add(A.step_acc + 1, 1);
+      rn_pool_add_initial_step(A.step_acc, log2Step);
 #endif
     }
   } else {
@@ -538,31 +529,19 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
       // pooled: one lane per chain adds the chain's share of the iteration's acceptance sum; rn_k_step_pool applies the update
       if (A.step_tuner == 0 && RN_LANE == 0) rn_pool_add(A.step_acc + it, rn_pool_quantise(rn_exp(a)));
 #else
-      if (A.step_tuner == 0) {  // DualAvg.update, DualAvg.scala:58-77
-        const double newAcceptanceProb = rn_exp(a);
-        daIter = daIter + 1;
-        const double avgErrorMultiplier = 1.0 / ((double)daIter + 10);
-        const double stepSizeMultiplier = rn_pow((double)daIter, -0.75);
-        avgError = ((1.0 - avgErrorMultiplier) * avgError + (avgErrorMultiplier * (A.delta - newAcceptanceProb)));
-        logStepSize = (shrinkageTarget - (avgError * sqrt((double)daIter) / 0.05));
-        logStepSizeBar = (stepSizeMultiplier * logStepSize + (1.0 - stepSizeMultiplier) * logStepSizeBar);
-        stepSize = rn_exp(logStepSize);
-      }
+      if (A.step_tuner == 0)
+        stepSize = rn_exp(rn_da_update(A, rn_exp(a), logStepSize, logStepSizeBar, avgError, shrinkageTarget, daIter));
 #endif
 #if RN_MASS_MAX >= 2
       if (A.mass_tuner == 2) {  // DenseMassMatrixTuner: WindowedMassMatrixTuner (MassMatrix.scala:147-164) over CovarianceEstimator
         win_j += 1;
-        if (!(win_j < A.skip_first || (A.total_warmup - win_j) < A.skip_last)) {
+        if (RN_IN_WINDOW(A, win_j)) {
           win_i += 1;
           est_samples += 1;
           RN_SYNC();
-          RN_FOR_LANES(i) {  // VarianceEstimator.update (MassMatrixEstimator.scala:69-83), diffs kept for the outer product
-            double mean = RN_AT(A.est_mean, i, c);
-            const double oldDiff = w.q[i] - mean;
-            mean += (oldDiff / (double)est_samples);
-            const double newDiff = w.q[i] - mean;
-            RN_AT(A.est_mean, i, c) = mean;
-            RN_AT(A.est_raw, i, c) += oldDiff * newDiff;
+          RN_FOR_LANES(i) {  // the differences are kept for the outer product
+            double oldDiff;
+            const double newDiff = rn_variance_update(A, c, i, w.q[i], est_samples, oldDiff);
             w.v[i] = oldDiff;
             w.v2[i] = newDiff;
           }
@@ -591,26 +570,7 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
             if (RN_LANE == 0) {  // choleskyUpperTriangular (MassMatrix.scala:76-117); `lower` borrows the estimator's
               double* lower = A.est_cov + c;  // covariance block, which was just reset and is zeroed again below
               const size_t ld = (size_t)A.chains;
-              int l = 0;
-              for (int i = 0; i < RN_N; i++)
-                for (int k = 0; k <= i; k++) {
-                  double sum = 0.0;
-                  for (int j = 0; j < k; j++) sum += lower[(size_t)((i * (i + 1)) / 2 + j) * ld] * lower[(size_t)((k * (k + 1)) / 2 + j) * ld];
-                  const double x = RN_AT(A.mass, i * RN_N + k, c) - sum;
-                  if (i == k)
-                    lower[(size_t)l * ld] = sqrt(x);
-                  else {
-                    const double diag = lower[(size_t)(((k + 1) * (k + 2)) / 2 - 1) * ld];
-                    lower[(size_t)l * ld] = (1.0 / diag * x);
-                  }
-                  l += 1;
-                }
-              l = 0;
-              for (int i = 0; i < RN_N; i++)
-                for (int k = 0; k < (RN_N - i); k++) {
-                  RN_AT(A.chol, l, c) = lower[(size_t)(((k + i) * (k + i + 1)) / 2 + i) * ld];
-                  l += 1;
-                }
+              rn_cholesky_upper(A, c, lower, ld);
               for (int e = 0; e < (RN_N * (RN_N + 1)) / 2; e++) lower[(size_t)e * ld] = 0.0;
             }
 #ifndef RN_HOST_EMULATION
@@ -618,15 +578,8 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
 #endif
             RN_SYNC();
             w.mass_kind = 2;
-            if (A.step_tuner == 0 && !RN_STEP_POOL) {  // stepSizeTuner.reset(), DualAvg.scala:17-21 (pooled: rn_k_step_pool)
-              const double ss = rn_exp(logStepSizeBar);
-              logStepSize = rn_log(ss);
-              logStepSizeBar = 0.0;
-              avgError = 0.0;
-              daIter = 0;
-              shrinkageTarget = rn_log(10 * ss);
-              stepSize = ss;
-            }
+            if (A.step_tuner == 0 && !RN_STEP_POOL)  // stepSizeTuner.reset() (pooled: rn_k_step_pool)
+              stepSize = rn_da_reset(logStepSize, logStepSizeBar, avgError, shrinkageTarget, daIter);
           }
           RN_SYNC();
         }
@@ -635,9 +588,11 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
       if (A.mass_tuner == 1) {  // DiagonalMassMatrixTuner, MassMatrix.scala:147-164
         win_j += 1;
         if (A.adaptation == 1) {  // pooled extension: per-chain Welford statistics of the window (see rn_k_pool_reduce / rn_k_pool_apply)
-          if (!(win_j < A.skip_first || (A.total_warmup - win_j) < A.skip_last)) {
+          if (RN_IN_WINDOW(A, win_j)) {
             win_i += 1;
-            RN_FOR_LANES(i) {  // the chain's Welford mean / M2 over this window (combined over chains at the window end)
+            // the chain's Welford mean / M2 over this window (combined over chains at the window end).  Not rn_variance_update:
+            // the second difference re-reads q after the store of the mean, which that helper does not do.
+            RN_FOR_LANES(i) {
               double mean = RN_AT(A.est_mean, i, c);
               const double od = w.q[i] - mean;
               mean += od / (double)win_i;
@@ -649,7 +604,7 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
               win_size = rn_d2i(win_size * A.win_expansion);
             }
           }
-        } else if (!(win_j < A.skip_first || (A.total_warmup - win_j) < A.skip_last)) {
+        } else if (RN_IN_WINDOW(A, win_j)) {
           win_i += 1;
           est_samples += 1;
           const bool window_end = (win_i == win_size);
@@ -675,15 +630,8 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
             win_i = 0;
             win_size = rn_d2i(win_size * A.win_expansion);
             w.mass_kind = 1;
-            if (A.step_tuner == 0 && !RN_STEP_POOL) {  // stepSizeTuner.reset(), DualAvg.scala:17-21 (pooled: rn_k_step_pool)
-              const double ss = rn_exp(logStepSizeBar);
-              logStepSize = rn_log(ss);
-              logStepSizeBar = 0.0;
-              avgError = 0.0;
-              daIter = 0;
-              shrinkageTarget = rn_log(10 * ss);
-              stepSize = ss;
-            }
+            if (A.step_tuner == 0 && !RN_STEP_POOL)  // stepSizeTuner.reset() (pooled: rn_k_step_pool)
+              stepSize = rn_da_reset(logStepSize, logStepSizeBar, avgError, shrinkageTarget, daIter);
           }
           RN_SYNC();
         }
@@ -733,84 +681,5 @@ RN_GLOBAL void rn_k_density(const double* RN_RESTRICT qin, double* RN_RESTRICT o
   RN_FOR_LANES(i) out[(size_t)(i + 1) * chains + c] = w.g[i];
   if (e && RN_LANE == 0) atomicOr(err, e);
 }
-
-#ifndef RN_HOST_EMULATION
-RN_GLOBAL void rn_k_transpose(const double* RN_RESTRICT src, double* RN_RESTRICT dst, int rows, int cols,
-                              long long src_ld, long long dst_ld, long long dst_off) {
-  // dst[c * dst_ld + dst_off + r] = src[r * src_ld + c]   (a block of `cols` chains out of src_ld)
-  __shared__ double tile[32][33];
-  const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
-  for (int j = threadIdx.y; j < 32; j += 8) {
-    const int r = r0 + j, c = c0 + threadIdx.x;
-    if (r < rows && c < cols) tile[j][threadIdx.x] = src[(size_t)r * (size_t)src_ld + c];
-  }
-  __syncthreads();
-  for (int j = threadIdx.y; j < 32; j += 8) {
-    const int c = c0 + j, r = r0 + threadIdx.x;
-    if (r < rows && c < cols) dst[(size_t)c * (size_t)dst_ld + (size_t)dst_off + r] = tile[threadIdx.x][j];
-  }
-}
-
-// =============================================================================================================
-// Pooled mass-matrix adaptation (RN_ADAPT_POOLED; an extension, not reference semantics): at a window end the
-// chains' Welford statistics of the window (mean_c, M2_c over L draws) are reduced over all chains of this GPU in two
-// passes -- pool[0] = number of chains and pool[1..n] = sum of the means, all-reduced over ranks by the host (NCCL),
-// then pool[n+1..2n] = sum of M2_c + L (mean_c - pooled mean)^2, all-reduced again -- and applied to every chain: one
-// shared diagonal mass matrix, statistics cleared, DualAvg restarted from each chain's averaged step size
-// (Driver.scala:75-80).
-// =============================================================================================================
-RN_GLOBAL void rn_k_pool_reduce(const RnArgs A, double* pool, int window_len, int pass) {
-  // One block per parameter; thread t adds chains t, t + 256, ... in order, then a fixed tree: the result does not depend
-  // on scheduling (no atomics).  pass 0: pool[1 + i] = sum over chains of the chain's window mean, pool[0] = chains.
-  // pass 1 (after the all-reduce of pass 0): pool[1 + n + i] = sum over chains of [M2_c + L (mean_c - mean)^2] -- Chan's
-  // combination of the chains' Welford statistics around the POOLED mean (no s2/n - mean^2 cancellation).
-  __shared__ double red[256];
-  const int i = (int)blockIdx.x;
-  const double gmean = pass ? pool[1 + i] / pool[0] : 0.0;
-  const double* mean = A.est_mean + (size_t)i * A.chains;
-  const double* m2 = A.est_raw + (size_t)i * A.chains;
-  double acc = 0.0;
-  for (int c = (int)threadIdx.x; c < A.chains; c += (int)blockDim.x) {
-    if (pass) {
-      const double d = mean[c] - gmean;
-      acc += m2[c] + (double)window_len * d * d;
-    } else {
-      acc += mean[c];
-    }
-  }
-  red[threadIdx.x] = acc;
-  __syncthreads();
-  for (int o = (int)blockDim.x / 2; o > 0; o >>= 1) {
-    if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    pool[1 + (pass ? RN_N : 0) + i] = red[0];
-    if (!pass && i == 0) pool[0] = (double)A.chains;
-  }
-}
-RN_GLOBAL void rn_k_pool_apply(const RnArgs A, const double* pool, int window_len) {
-  const int c = (int)(blockIdx.x * blockDim.x + threadIdx.x);
-  if (c >= A.chains) return;
-  const double cnt = pool[0] * (double)window_len;  // draws of the window over all chains of all ranks
-  for (int i = 0; i < RN_N; i++) {
-    const double var = pool[1 + RN_N + i] / cnt;
-    if (!(var > 0.0)) A.st_err[c] |= 2;
-    RN_AT(A.mass, i, c) = var;
-    RN_AT(A.est_mean, i, c) = 0.0;
-    RN_AT(A.est_raw, i, c) = 0.0;
-  }
-  if (A.step_tuner == 0) {  // stepSizeTuner.reset(), DualAvg.scala:17-21
-    const double ss = rn_exp(RN_AT(A.da, 2, c));
-    RN_AT(A.da, 0, c) = ss;
-    RN_AT(A.da, 1, c) = rn_log(ss);
-    RN_AT(A.da, 2, c) = 0.0;
-    RN_AT(A.da, 3, c) = 0.0;
-    RN_AT(A.da, 4, c) = rn_log(10 * ss);
-    A.da_iter[c] = 0;
-  }
-}
-
-#endif  // !RN_HOST_EMULATION
 
 #endif  // RN_SAMPLER_WPC_CUH

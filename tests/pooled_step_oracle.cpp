@@ -1,5 +1,5 @@
 /* tests/pooled_step_oracle.cpp -- TEST INFRASTRUCTURE ONLY: the oracle's restatement of the two pooled adaptation modes,
- * pooled step sizes (rn_config.step_adaptation == RN_ADAPT_POOLED, rainier_b200/csrc/rn_step_pool.cuh) and pooled mass
+ * pooled step sizes (rn_config.step_adaptation == RN_ADAPT_POOLED, rainier_b200/csrc/rn_sampler_common.cuh) and pooled mass
  * windows (rn_config.adaptation == RN_ADAPT_POOLED, rn_k_pool_reduce / rn_k_pool_apply).  The reference adapts per chain;
  * these extensions share state over all chains, so the chains can no longer run one after another: a lockstep driver runs
  * iterations outer, chains inner.

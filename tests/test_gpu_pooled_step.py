@@ -1,5 +1,5 @@
 """
-Pooled step-size adaptation on the device (rn_config.step_adaptation = RN_ADAPT_POOLED, rn_step_pool.cuh): against the
+Pooled step-size adaptation on the device (rn_config.step_adaptation = RN_ADAPT_POOLED, rn_sampler_common.cuh): against the
 oracle's lockstep restatement (tests/pooled_step_oracle.cpp), across chain orders, kernel families (thread per chain, warp
 per chain, the DMMA lockstep path), together with pooled mass windows, and through the one-call rn_sample path.
 """
