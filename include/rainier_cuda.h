@@ -115,7 +115,9 @@ typedef struct rn_config {
   /* extensions (not in the reference) */
   int32_t adaptation;        /* RN_ADAPT_PER_CHAIN (parity with the reference, default) or RN_ADAPT_POOLED:
                                 mass-matrix windows pool Welford statistics over all chains (and, when a
-                                communicator is attached, all ranks) */
+                                communicator is attached, all ranks).  RN_MASS_DIAGONAL pools the variances,
+                                RN_MASS_DENSE the covariances (one shared matrix, factored once per window);
+                                other tuners are refused */
   int32_t math_mode;         /* RN_MATH_PARITY: no FMA contraction, the reference's operation order;
                                 RN_MATH_FAST: FMA contraction allowed */
   int32_t gradient_mode;     /* RN_GRAD_AUTO: use the RIR's symbolic gradient outputs when present, else adjoint */

@@ -1877,6 +1877,7 @@ std::string emit_source(const Program& P, const EmitOptions& opt) {
   os << "#define RN_MASS_MAX " << opt.mass_max << "\n";
   os << "#define RN_ENABLE_EHMC " << (opt.enable_ehmc ? 1 : 0) << "\n";
   if (opt.step_pool) os << "#define RN_STEP_POOL 1\n";
+  if (opt.mass_pool) os << "#define RN_MASS_POOL 1\n";
   if (opt.fast_math) os << "#define RN_FAST_MATH 1\n";
   if (opt.backend == 1) {
     os << "#define RN_WPC_K " << std::max(1, opt.wpc_k) << "\n";

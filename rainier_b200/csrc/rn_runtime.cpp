@@ -156,9 +156,10 @@ struct KernelKey {
   int mass_max, backend;
   int block = 0;  // thread-per-chain: CTA size the module was compiled for (RN_BLOCK_DIM), 0 = any (emit / density-only uses)
   bool step_pool = false;  // pooled step-size adaptation compiled in (RN_STEP_POOL)
+  bool mass_pool = false;  // pooled dense mass windows compiled in (RN_MASS_POOL)
   bool operator<(const KernelKey& o) const {
-    return std::tie(adjoint, fast, ehmc, mass_max, backend, block, step_pool) <
-           std::tie(o.adjoint, o.fast, o.ehmc, o.mass_max, o.backend, o.block, o.step_pool);
+    return std::tie(adjoint, fast, ehmc, mass_max, backend, block, step_pool, mass_pool) <
+           std::tie(o.adjoint, o.fast, o.ehmc, o.mass_max, o.backend, o.block, o.step_pool, o.mass_pool);
   }
 };
 // SMs of a device; handles without one (emit / compile only) assume an H100 SXM's 132
@@ -185,10 +186,12 @@ struct Kernel {
   std::vector<char> cubin;
   CUmodule mod = nullptr;
   CUfunction k_init = nullptr, k_iter = nullptr, k_warmup = nullptr, k_density = nullptr, k_transpose = nullptr, k_pool_reduce = nullptr,
-             k_pool_apply = nullptr, k_diag_chain = nullptr, k_diag_reduce = nullptr, k_step_pool = nullptr;
+             k_pool_apply = nullptr, k_diag_chain = nullptr, k_diag_reduce = nullptr, k_step_pool = nullptr,
+             k_pool_reduce_dense = nullptr, k_pool_factor = nullptr, k_pool_apply_dense = nullptr;
   const Program* prog = nullptr;
   int backend = 0;            // 0 thread per chain, 1 warp per chain
   bool step_pool = false;     // rn_k_step_pool compiled in (pooled step-size adaptation)
+  bool mass_pool = false;     // rn_k_pool_reduce_dense / rn_k_pool_factor / rn_k_pool_apply_dense compiled in (pooled dense windows)
   unsigned tpc_block = 0;     // backend 0: the CTA size this module was compiled for (0: reads blockDim.x)
   int wpc_smem_doubles = 0;   // per-warp dynamic shared memory (backend 1)
   int warps_per_cta = 4;      // backend 1: CHAINS per CTA (each owned by wpc_k warps)
@@ -274,6 +277,7 @@ static KernelKey key_for(const rn_model* m, const rn_config* cfg) {
   k.fast = cfg && cfg->math_mode == RN_MATH_FAST;
   k.ehmc = cfg && cfg->sampler == RN_SAMPLER_EHMC;
   k.step_pool = cfg && cfg->step_adaptation == RN_ADAPT_POOLED;
+  k.mass_pool = cfg && cfg->adaptation == RN_ADAPT_POOLED && cfg->mass_tuner == RN_MASS_DENSE;
   k.mass_max = 0;
   if (cfg) {
     if (cfg->mass_tuner == RN_MASS_DIAGONAL) k.mass_max = 1;
@@ -322,12 +326,14 @@ static int get_kernel(rn_model* m, const rn_config* cfg, Kernel** out, std::stri
   eo.mass_max = key.mass_max;
   eo.enable_ehmc = key.ehmc;
   eo.step_pool = key.step_pool;
+  eo.mass_pool = key.mass_pool;
   eo.target_base = m->target_base;
   eo.target_pitch = m->target_pitch;
   if (eo.backend == 1 && P->symbolic && P->n_params > 96)
     return fail(RN_E_UNSUPPORTED, "warp-per-chain with a symbolic gradient keeps n+1 accumulators in registers; use RN_GRAD_ADJOINT for n > 96");
   K->backend = eo.backend;
   K->step_pool = key.step_pool;
+  K->mass_pool = key.mass_pool;
   K->tpc_block = (unsigned)key.block;
   if (eo.backend == 0) {  // rn_sampler.cuh: RN_TS_DOUBLES * 8 + RN_TS_INTS * 4
     const unsigned n = P->n_params;
@@ -534,6 +540,11 @@ static int load_kernel(const Api* A, rn_model* m, Kernel* K) {
   CU(A->cuModuleGetFunction(&K->k_diag_chain, K->mod, "rn_k_diag_chain"));
   CU(A->cuModuleGetFunction(&K->k_diag_reduce, K->mod, "rn_k_diag_reduce"));
   if (K->step_pool) CU(A->cuModuleGetFunction(&K->k_step_pool, K->mod, "rn_k_step_pool"));
+  if (K->mass_pool) {
+    CU(A->cuModuleGetFunction(&K->k_pool_reduce_dense, K->mod, "rn_k_pool_reduce_dense"));
+    CU(A->cuModuleGetFunction(&K->k_pool_factor, K->mod, "rn_k_pool_factor"));
+    CU(A->cuModuleGetFunction(&K->k_pool_apply_dense, K->mod, "rn_k_pool_apply_dense"));
+  }
   if (K->backend == 1) {
     const int bytes = (int)K->smem_bytes();
     for (CUfunction f : {K->k_init, K->k_iter, K->k_density})
@@ -1002,7 +1013,7 @@ struct rn_sampler {
   CUdeviceptr d_trace = 0;  // optional test instrumentation, [warmup+iterations][4][chains]
   size_t trace_iters = 0, trace_pos = 0;
   rn_comm* comm = nullptr;
-  CUdeviceptr d_pool = 0;  // [2n+1] pooled window statistics (RN_ADAPT_POOLED)
+  CUdeviceptr d_pool = 0;  // pooled window statistics (RN_ADAPT_POOLED): [2n+1], dense [1+n+n^2] + factor scratch
   CUdeviceptr d_step = 0;  // int64 [2 + warmup]: K, C, Q_t of pooled step-size adaptation (rn_sampler_common.cuh), zeroed at create
   // device time of the sampling phase (Stats.gradientTimes / iterationTimes, Stats.scala:8-9): events bracket every
   // batch of phase-1 launches; closed spans are summed when the stats are read
@@ -1096,6 +1107,13 @@ int iterations_to_window_end(const rn_sampler* s, int limit) {
   return limit;
 }
 
+// doubles of the pooled window buffer behind the arena: [2n+1]; pooled dense windows (rn_sampler_common.cuh, RN_MASS_POOL)
+// [1 + n + n^2] and the factor scratch (lower and upper packed factors, one flag)
+size_t pool_doubles(const rn_sampler* s) {
+  const size_t n = s->m->n_params;
+  return s->K->mass_pool ? 1 + n + n * n + n * (n + 1) + 1 : 2 * n + 1;
+}
+
 int check_config(const rn_model* m, const rn_config* c, int chains) {
   if (!c) return fail(RN_E_INVALID, "null config");
   if (c->struct_size != (int32_t)sizeof(rn_config)) return fail(RN_E_INVALID, "rn_config.struct_size mismatch");
@@ -1121,8 +1139,8 @@ int check_config(const rn_model* m, const rn_config* c, int chains) {
       return fail(RN_E_UNSUPPORTED, "dense mass matrix on the thread-per-chain kernels is supported for n <= 64 (use RN_BACKEND_WARP)");
     if (warp && m->n_params > 512) return fail(RN_E_UNSUPPORTED, "dense mass matrix supported for n <= 512");
   }
-  if (c->adaptation == RN_ADAPT_POOLED && c->mass_tuner != RN_MASS_DIAGONAL)
-    return fail(RN_E_UNSUPPORTED, "pooled adaptation is implemented for the diagonal mass-matrix tuner");
+  if (c->adaptation == RN_ADAPT_POOLED && c->mass_tuner != RN_MASS_DIAGONAL && c->mass_tuner != RN_MASS_DENSE)
+    return fail(RN_E_UNSUPPORTED, "pooled adaptation is implemented for the diagonal and dense mass-matrix tuners");
   if (c->step_adaptation != RN_ADAPT_PER_CHAIN && c->step_adaptation != RN_ADAPT_POOLED)
     return fail(RN_E_INVALID, "step_adaptation must be RN_ADAPT_PER_CHAIN or RN_ADAPT_POOLED");
   if (c->step_adaptation == RN_ADAPT_POOLED && c->step_size_tuner == RN_STEP_STATIC)
@@ -1181,7 +1199,7 @@ int rn_sampler_create(rn_model* m, const rn_config* cfg, const int64_t* seeds, i
                o_srf = ar.take(3 * C * 4);
   s->stats_bytes = ar.off - s->stats_off;
   s->arena_bytes = ar.off;
-  const size_t pool_off = (s->arena_bytes + 255) & ~(size_t)255, need = pool_off + (2 * n + 1) * 8;
+  const size_t pool_off = (s->arena_bytes + 255) & ~(size_t)255, need = pool_off + pool_doubles(s.get()) * 8;
   if (m->spare_arena && m->spare_arena_bytes >= need) {
     s->arena = m->spare_arena;
     s->arena_alloc = m->spare_arena_bytes;
@@ -1191,7 +1209,7 @@ int rn_sampler_create(rn_model* m, const rn_config* cfg, const int64_t* seeds, i
     CU(A->cuMemAlloc(&s->arena, need));
     s->arena_alloc = need;
   }
-  s->d_pool = s->arena + pool_off;  // [2n+1] pooled window statistics live behind the chain state
+  s->d_pool = s->arena + pool_off;  // the pooled window statistics live behind the chain state
   CU(A->cuMemsetD8Async(s->arena, 0, s->arena_bytes, s->stream));
 
   RnArgs& a = s->args;
@@ -1331,8 +1349,46 @@ static int comm_allreduce(const Api* A, rn_sampler* s, CUdeviceptr buf, size_t c
   return RN_OK;
 }
 
+// pooled dense window end: pass 0 (rn_k_pool_reduce), all-reduce of pool[0..n]; pass 1 over the n^2 co-moments
+// (rn_k_pool_reduce_dense), all-reduce of them; one factorisation of the pooled matrix (rn_k_pool_factor) on every rank;
+// broadcast of matrix and factor to every chain (rn_k_pool_apply_dense)
+static int pool_window_dense(const Api* A, rn_sampler* s, int window_len) {
+  const size_t n = s->m->n_params;
+  CU(A->cuMemsetD8Async(s->d_pool, 0, (1 + n + n * n) * 8, s->stream));
+  CUdeviceptr pool = s->d_pool;
+  int wl = window_len, ps = 0;
+  {
+    void* params[] = {&s->args, &pool, &wl, &ps};
+    CU(A->cuLaunchKernel(s->K->k_pool_reduce, (unsigned)n, 1, 1, 256, 1, 1, 0, s->stream, params, nullptr));
+    s->launches++;
+  }
+  int rc = comm_allreduce(A, s, s->d_pool, n + 1, 8 /*ncclFloat64*/);
+  if (rc) return rc;
+  {
+    void* params[] = {&s->args, &pool, &wl};
+    CU(A->cuLaunchKernel(s->K->k_pool_reduce_dense, (unsigned)(n * n), 1, 1, 256, 1, 1, 0, s->stream, params, nullptr));
+    s->launches++;
+  }
+  rc = comm_allreduce(A, s, s->d_pool + (1 + n) * 8, n * n, 8 /*ncclFloat64*/);
+  if (rc) return rc;
+  {
+    void* params[] = {&pool, &wl};
+    const unsigned threads = (unsigned)std::min<size_t>(512, (n + 31) / 32 * 32);
+    CU(A->cuLaunchKernel(s->K->k_pool_factor, 1, 1, 1, threads, 1, 1, 0, s->stream, params, nullptr));
+    s->launches++;
+  }
+  {
+    void* params[] = {&s->args, &pool, &wl};
+    CU(A->cuLaunchKernel(s->K->k_pool_apply_dense, (unsigned)((s->chains + 127) / 128), (unsigned)std::min<size_t>(n, 64), 1, 128, 1, 1,
+                         0, s->stream, params, nullptr));
+    s->launches++;
+  }
+  return RN_OK;
+}
+
 static int pool_window(const Api* A, rn_sampler* s, int window_len) {
   const size_t n = s->m->n_params;
+  if (s->K->mass_pool) return pool_window_dense(A, s, window_len);
   CU(A->cuMemsetD8Async(s->d_pool, 0, (2 * n + 1) * 8, s->stream));
   // two passes (pooled mean, then Chan's combination of the chains' M2 around it), each a deterministic reduction over this
   // GPU's chains followed by one small all-reduce over the ranks
@@ -1372,7 +1428,8 @@ static int run_phase(const Api* A, rn_sampler* s, int phase, int iterations, dou
                      int chain_end = -1) {
   if (chain_end < 0) chain_end = s->chains;
   const int per_launch = s->cfg.launch_iterations > 0 ? s->cfg.launch_iterations : 1000;
-  const bool pooled = phase == 0 && s->cfg.adaptation == RN_ADAPT_POOLED && s->cfg.mass_tuner == RN_MASS_DIAGONAL;
+  const bool pooled = phase == 0 && s->cfg.adaptation == RN_ADAPT_POOLED &&
+                      (s->cfg.mass_tuner == RN_MASS_DIAGONAL || s->cfg.mass_tuner == RN_MASS_DENSE);
   const bool step_pooled = phase == 0 && s->K->step_pool;
   int done = 0;
   if (phase == 1 && iterations > 0) {

@@ -757,11 +757,21 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
           // end (rn_k_pool_reduce / rn_k_pool_apply) -- launches are cut at window ends in this mode
           if (RN_IN_WINDOW(A, win_j)) {
             win_i += 1;
+#if RN_MASS_POOL
+            // pooled dense: the window's Welford mean and co-moment (CovarianceEstimator.update, :28-41); the window end is
+            // rn_k_pool_reduce_dense / rn_k_pool_factor / rn_k_pool_apply_dense
+            double oldDiff[RN_N], newDiff[RN_N];
+            RN_UNROLL
+            for (int i = 0; i < RN_N; i++) newDiff[i] = rn_variance_update(A, c, i, s.q[i], win_i, oldDiff[i]);
+            for (int j = 0; j < RN_N; j++)
+              for (int k = 0; k < RN_N; k++) RN_AT(A.est_cov, j * RN_N + k, c) += newDiff[j] * oldDiff[k];
+#else
             RN_UNROLL
             for (int i = 0; i < RN_N; i++) {  // the chain's Welford mean / M2 over this window
               double oldDiff;
               rn_variance_update(A, c, i, s.q[i], win_i, oldDiff);
             }
+#endif
             if (win_i == win_size) {
               win_i = 0;
               win_size = rn_d2i(win_size * A.win_expansion);

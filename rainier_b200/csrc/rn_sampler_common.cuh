@@ -12,6 +12,9 @@
 #ifndef RN_STEP_POOL
 #define RN_STEP_POOL 0 /* 1: pooled step-size adaptation (rn_k_step_pool below) */
 #endif
+#ifndef RN_MASS_POOL
+#define RN_MASS_POOL 0 /* 1: pooled dense mass windows (rn_k_pool_reduce_dense / rn_k_pool_factor / rn_k_pool_apply_dense below) */
+#endif
 // field `field` of chain c in a [field][chains] (SoA) array
 #define RN_AT(ptr, field, c) (ptr)[(size_t)(field) * (size_t)A.chains + (size_t)(c)]
 
@@ -232,6 +235,96 @@ RN_GLOBAL void rn_k_pool_apply(const RnArgs A, const double* pool, int window_le
   if (A.step_tuner == 0)
     RN_AT(A.da, 0, c) = rn_da_reset(RN_AT(A.da, 1, c), RN_AT(A.da, 2, c), RN_AT(A.da, 3, c), RN_AT(A.da, 4, c), A.da_iter[c]);
 }
+
+#if RN_MASS_POOL
+// ---- pooled dense mass windows (DenseMassMatrixTuner with RN_ADAPT_POOLED; an extension, not reference semantics) ---------
+// The chains keep their window mean and co-moment C2[j][k] += newDiff[j] * oldDiff[k] (CovarianceEstimator.update,
+// MassMatrixEstimator.scala:22-36) with the position in the window as the count.  At a window end pass 0 is rn_k_pool_reduce's
+// (pool[0] = chains, pool[1..n] = sum of the means), then pool[1 + n + j n + k] = sum over chains of
+// C2_c[j][k] + (L d_c[j]) d_c[k], d_c = mean_c - pooled mean, over all n^2 entries (C2 is not exactly symmetric and the
+// velocity reads the full matrix).  M = S / (C L), with the diagonal kernels' association throughout, so M's diagonal is
+// the pooled diagonal tuner's variance bit for bit.  rn_k_pool_factor factors M once, in one CTA, into the scratch behind
+// the pool; rn_k_pool_apply_dense broadcasts M and the factor to every chain.
+// pool layout: [0] C | [1, 1+n) sum of means | [1+n, 1+n+n^2) S | lower factor [n(n+1)/2] | upper factor [n(n+1)/2] | flag
+#define RN_POOL_TRI ((RN_N * (RN_N + 1)) / 2)
+#define RN_POOL_FACTOR_OFF (1 + RN_N + RN_N * RN_N)
+RN_GLOBAL void rn_k_pool_reduce_dense(const RnArgs A, double* pool, int window_len) {
+  // one block per entry e = j n + k, rn_k_pool_reduce's order: thread t adds chains t, t + 256, ..., then a halving tree
+  __shared__ double red[256];
+  const int e = (int)blockIdx.x, j = e / RN_N, k = e % RN_N;
+  const double gj = pool[1 + j] / pool[0], gk = pool[1 + k] / pool[0];
+  const double* mj = A.est_mean + (size_t)j * A.chains;
+  const double* mk = A.est_mean + (size_t)k * A.chains;
+  const double* cov = A.est_cov + (size_t)e * A.chains;
+  double acc = 0.0;
+  for (int c = (int)threadIdx.x; c < A.chains; c += (int)blockDim.x) {
+    const double dj = mj[c] - gj, dk = mk[c] - gk;
+    acc += cov[c] + (double)window_len * dj * dk;
+  }
+  red[threadIdx.x] = acc;
+  __syncthreads();
+  for (int o = (int)blockDim.x / 2; o > 0; o >>= 1) {
+    if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) pool[1 + RN_N + e] = red[0];
+}
+// choleskyUpperTriangular (MassMatrix.scala:76-117) of M = S / (C L), column by column: for column k every row i >= k
+// forms x_i = M[i][k] - sum_{j<k} L[i][j] L[k][j] with its own sequential sum from j = 0, then L[k][k] = sqrt(x_k) and
+// L[i][k] = 1 / L[k][k] * x_i.  Each entry is the operation sequence of rn_cholesky_upper, so parity builds give its bits.
+// Flag = 1 when M has an element equal to 0.0 (MassMatrix.scala:16) or a pivot is not > 0.  One CTA, thread t owns rows
+// t, t + blockDim.x, ...; the factor stays in global memory (a packed factor at n = 512 does not fit in shared memory).
+RN_GLOBAL void rn_k_pool_factor(double* pool, int window_len) {
+  __shared__ double xs[RN_N];
+  const double cnt = pool[0] * (double)window_len;
+  const double* S = pool + 1 + RN_N;
+  double* lower = pool + RN_POOL_FACTOR_OFF;
+  double* upper = lower + RN_POOL_TRI;
+  int bad = 0;
+  for (int e = (int)threadIdx.x; e < RN_N * RN_N; e += (int)blockDim.x)
+    if (S[e] / cnt == 0.0) bad = 1;
+  for (int k = 0; k < RN_N; k++) {
+    for (int i = k + (int)threadIdx.x; i < RN_N; i += (int)blockDim.x) {
+      double sum = 0.0;
+      for (int j = 0; j < k; j++) sum += lower[(i * (i + 1)) / 2 + j] * lower[(k * (k + 1)) / 2 + j];
+      xs[i] = S[i * RN_N + k] / cnt - sum;
+    }
+    __syncthreads();
+    const double diag = sqrt(xs[k]);
+    if (threadIdx.x == 0 && !(diag > 0.0)) bad = 1;
+    for (int i = k + (int)threadIdx.x; i < RN_N; i += (int)blockDim.x) {
+      const double v = i == k ? diag : (1.0 / diag * xs[i]);
+      lower[(i * (i + 1)) / 2 + k] = v;
+      upper[k * RN_N - (k * (k - 1)) / 2 + (i - k)] = v;  // row k of the packed upper factor, column i
+    }
+    __syncthreads();
+  }
+  bad = __syncthreads_or(bad);
+  if (threadIdx.x == 0) upper[RN_POOL_TRI] = bad ? 1.0 : 0.0;
+}
+// every chain: M (mass, [n^2][chains]) and the packed upper factor (chol, [n(n+1)/2][chains]), estimator cleared, error flag
+// 2 where rn_k_pool_factor flagged, DualAvg restarted as in rn_k_pool_apply.  x: chains; y: entries strided by gridDim.y.
+RN_GLOBAL void rn_k_pool_apply_dense(const RnArgs A, const double* pool, int window_len) {
+  const int c = (int)(blockIdx.x * blockDim.x + threadIdx.x);
+  if (c >= A.chains) return;
+  const double cnt = pool[0] * (double)window_len;
+  const double* S = pool + 1 + RN_N;
+  const double* upper = pool + RN_POOL_FACTOR_OFF + RN_POOL_TRI;
+  for (int e = (int)blockIdx.y; e < RN_N * RN_N; e += (int)gridDim.y) {
+    RN_AT(A.mass, e, c) = S[e] / cnt;
+    RN_AT(A.est_cov, e, c) = 0.0;
+  }
+  for (int e = (int)blockIdx.y; e < RN_POOL_TRI; e += (int)gridDim.y) RN_AT(A.chol, e, c) = upper[e];
+  for (int i = (int)blockIdx.y; i < RN_N; i += (int)gridDim.y) {
+    RN_AT(A.est_mean, i, c) = 0.0;
+    RN_AT(A.est_raw, i, c) = 0.0;
+  }
+  if (blockIdx.y != 0) return;
+  if (upper[RN_POOL_TRI] != 0.0) A.st_err[c] |= 2;
+  if (A.step_tuner == 0)
+    RN_AT(A.da, 0, c) = rn_da_reset(RN_AT(A.da, 1, c), RN_AT(A.da, 2, c), RN_AT(A.da, 3, c), RN_AT(A.da, 4, c), A.da_iter[c]);
+}
+#endif  // RN_MASS_POOL
 #endif  // !RN_HOST_EMULATION
 
 #endif  // RN_SAMPLER_COMMON_CUH

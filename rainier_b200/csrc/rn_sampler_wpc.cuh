@@ -535,6 +535,32 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
 #if RN_MASS_MAX >= 2
       if (A.mass_tuner == 2) {  // DenseMassMatrixTuner: WindowedMassMatrixTuner (MassMatrix.scala:147-164) over CovarianceEstimator
         win_j += 1;
+#if RN_MASS_POOL
+        // pooled extension: the chain's Welford mean and co-moment of the window (the count is the position in the window);
+        // rn_k_pool_reduce / rn_k_pool_reduce_dense / rn_k_pool_factor / rn_k_pool_apply_dense do the window end
+        if (RN_IN_WINDOW(A, win_j)) {
+          win_i += 1;
+          RN_SYNC();
+          RN_FOR_LANES(i) {
+            double mean = RN_AT(A.est_mean, i, c);
+            const double od = w.q[i] - mean;
+            mean += od / (double)win_i;
+            RN_AT(A.est_mean, i, c) = mean;
+            const double nd = w.q[i] - mean;
+            RN_AT(A.est_raw, i, c) += od * nd;
+            w.v[i] = od;
+            w.v2[i] = nd;
+          }
+          RN_SYNC();
+          for (int e = RN_LANE; e < RN_N * RN_N; e += RN_G)  // CovarianceEstimator.update, :28-41
+            RN_AT(A.est_cov, e, c) += w.v2[e / RN_N] * w.v[e % RN_N];
+          if (win_i == win_size) {
+            win_i = 0;
+            win_size = rn_d2i(win_size * A.win_expansion);
+          }
+          RN_SYNC();
+        }
+#else
         if (RN_IN_WINDOW(A, win_j)) {
           win_i += 1;
           est_samples += 1;
@@ -583,6 +609,7 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
           }
           RN_SYNC();
         }
+#endif  // RN_MASS_POOL
       }
 #endif
       if (A.mass_tuner == 1) {  // DiagonalMassMatrixTuner, MassMatrix.scala:147-164

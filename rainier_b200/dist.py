@@ -6,7 +6,8 @@ rainier-sampler/.../sampler/Driver.scala:13-17), so the sampling path needs NO c
 chain block `chain_block(total, r, world)` with the same per-chain seeds a single process would use, and results are
 rank-local until gathered.  The only exchange step is optional and warmup-only: pooling mass-matrix window statistics
 over all chains of all ranks (RN_ADAPT_POOLED) -- two sum all-reduces per window of the chains' Welford statistics: first
-{chains, sum of the chains' window means} (n+1 doubles), then sum of M2_c + L (mean_c - pooled mean)^2 (n doubles).
+{chains, sum of the chains' window means} (n+1 doubles), then sum of M2_c + L (mean_c - pooled mean)^2 (n doubles), or
+with the dense tuner the n^2 sums of C2_c[j][k] + L d_c[j] d_c[k] (`combine_welford_dense`).
 
 torch.distributed is used purely as plumbing (NCCL on GPUs, gloo in the CPU tests).
 """
@@ -44,6 +45,18 @@ def combine_welford(n, mean, m2):
     k = mean.shape[0]
     g = mean.sum(axis=0) / k
     return (m2 + n * (mean - g) ** 2).sum(axis=0) / (k * n)
+
+
+def combine_welford_dense(n, mean, cov):
+    """Host mirror of the pooled dense window reduction (rn_k_pool_reduce pass 0, rn_k_pool_reduce_dense): chains (or ranks)
+    each hold n draws with mean `mean[k]` ([K][d]) and co-moment `cov[k]` ([K][d][d], the sum of products of deviations from
+    their own mean); the pooled population covariance [d][d] is [sum_k cov[k] + n (mean[k] - g)(mean[k] - g)^T] / (K n)
+    around the pooled mean g.  With a communicator the library all-reduces {K, sum of the means} (d + 1 doubles), then the
+    d^2 sums, and factors the result once per window."""
+    mean, cov = np.asarray(mean, dtype=np.float64), np.asarray(cov, dtype=np.float64)
+    k = mean.shape[0]
+    d = mean - mean.sum(axis=0) / k
+    return (cov + n * d[:, :, None] * d[:, None, :]).sum(axis=0) / (k * n)
 
 
 def allreduce_window_stats(stats, group=None):
