@@ -238,6 +238,23 @@ int rn_sampler_stats(rn_sampler* s, rn_chain_stats* stats, double* mass, double*
  * over a DEVICE-resident sample block, reduced on the device (only n*2 numbers cross PCIe).  layout 0 =
  * [iterations][n][chains] (as rn_sampler_run writes it), 1 = [chains][iterations][n].  out: host [n][2]. */
 int rn_sampler_diagnostics(rn_sampler* s, const double* d_samples, int iterations, int layout, double* out);
+/* Trace.thin(thin).diagnostics over every sampling iteration rn_sampler_run performs after this call, accumulated on
+ * the device as the draws are produced: no sample block is kept, and rn_sampler_run may be given d_samples == NULL.
+ * Warmup draws are never tracked.  Calling it again restarts the accumulation.  thin >= 1.
+ * Kept draws are those whose index among the tracked draws is a multiple of thin (index 0: the first draw after this
+ * call), whatever the split into rn_sampler_run calls; any split gives bit-identical results.
+ * Device memory, independent of the number of iterations: the state, 201 doubles per (parameter, chain), and the finish's
+ * scratch, 8 doubles per (parameter, chain), both allocated by the first call and freed by rn_sampler_destroy.  With
+ * d_samples == NULL, rn_sampler_run also keeps a scratch of one launch's draws, launch_iterations * n * chains doubles
+ * (cfg->launch_iterations, 0 = 1000): lower launch_iterations to bound it.  The accumulation launches are not counted by
+ * rn_sampler_launches and their time is not in rn_chain_stats' time fields. */
+int rn_sampler_track_diagnostics(rn_sampler* s, int thin);
+/* out: host [n][2] = rHat, effectiveSampleSize over the tracked draws of every chain.  With a communicator attached this
+ * covers every chain of every rank and is a collective: every rank calls it, and every rank gets the same numbers or
+ * the same error code.  RN_E_INVALID: called before rn_sampler_track_diagnostics (on any rank), fewer than 2 chains in
+ * total, fewer than 2 kept draws, or kept counts that differ between ranks.  Its two all-reduces are not counted by
+ * rn_sampler_comm_stats. */
+int rn_sampler_tracked_diagnostics(rn_sampler* s, double* out);
 /* the CUstream the sampler launches on (for CUDA-event timing by the caller) */
 void* rn_sampler_stream(rn_sampler* s);
 /* number of kernel launches issued so far on this sampler */

@@ -201,6 +201,17 @@ JNIEXPORT void JNICALL Java_com_stripe_rainier_cuda_Native_optimize(JNIEnv* env,
   out_doubles(env, x, vx.data(), vx.size());
   if (info) env->SetIntArrayRegion(info, 0, (jsize)vi.size(), (const jint*)vi.data());
 }
+// ---- Trace.thin(thin).diagnostics tracked while a staged sampler runs (rn_sampler_track_diagnostics) ----
+// def samplerTrackDiagnostics(sampler: Long, thin: Int): Unit
+JNIEXPORT void JNICALL Java_com_stripe_rainier_cuda_Native_samplerTrackDiagnostics(JNIEnv* env, jclass, jlong s, jint thin) {
+  if (rn_sampler_track_diagnostics((rn_sampler*)(intptr_t)s, thin) != RN_OK) throw_last(env);
+}
+// def samplerTrackedDiagnostics(sampler: Long, out: Array[Double] /* [n][2] = rHat, ess */): Unit   (a collective with a communicator)
+JNIEXPORT void JNICALL Java_com_stripe_rainier_cuda_Native_samplerTrackedDiagnostics(JNIEnv* env, jclass, jlong s, jdoubleArray out) {
+  std::vector<double> vo((size_t)env->GetArrayLength(out));
+  if (rn_sampler_tracked_diagnostics((rn_sampler*)(intptr_t)s, vo.data()) != RN_OK) return throw_last(env);
+  out_doubles(env, out, vo.data(), vo.size());
+}
 JNIEXPORT jstring JNICALL Java_com_stripe_rainier_cuda_Native_lastError(JNIEnv* env, jclass) {
   return env->NewStringUTF(rn_last_error());
 }

@@ -72,6 +72,8 @@ def lib():
         L.rn_sampler_positions.argtypes = [C.c_void_p, C.c_void_p]
         L.rn_sampler_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.rn_sampler_diagnostics.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+        L.rn_sampler_track_diagnostics.argtypes = [C.c_void_p, C.c_int]
+        L.rn_sampler_tracked_diagnostics.argtypes = [C.c_void_p, C.c_void_p]
         L.rn_sampler_stream.argtypes = [C.c_void_p]
         L.rn_sampler_stream.restype = C.c_void_p
         L.rn_sampler_launches.argtypes = [C.c_void_p]
@@ -764,6 +766,18 @@ class CudaSampler:
         Returns an array [n][2] = (rHat, effectiveSampleSize)."""
         out = np.empty((self.model.nVars, 2), dtype=np.float64)
         _check(lib().rn_sampler_diagnostics(self.h, C.c_void_p(d_samples), int(iterations), int(layout), out.ctypes.data))
+        return out
+
+    def track_diagnostics(self, thin=1):
+        """Trace.thin(thin).diagnostics over every sampling iteration run() performs from now on, accumulated on the device
+        as the draws are produced (run() may then be given no sample block).  Calling it again restarts the accumulation."""
+        _check(lib().rn_sampler_track_diagnostics(self.h, int(thin)))
+
+    def tracked_diagnostics(self):
+        """[n][2] = (rHat, effectiveSampleSize) over the tracked draws; with a communicator attached, over every chain of
+        every rank (a collective: every rank calls it)"""
+        out = np.empty((self.model.nVars, 2), dtype=np.float64)
+        _check(lib().rn_sampler_tracked_diagnostics(self.h, out.ctypes.data))
         return out
 
     def positions(self):

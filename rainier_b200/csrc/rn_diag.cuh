@@ -8,6 +8,8 @@
 //                     chain's series (summed over iterations in the reference's sequential order), reduced over the 128
 //                     chains of the block in a fixed order.
 //   rn_k_diag_reduce  fixed-shape tree sums over blocks / chains (deterministic), optionally of squared deviations.
+//   rn_k_diag_accum   tracked diagnostics: the same sums carried from one sampling launch to the next (no sample block).
+//   rn_k_diag_terms   tracked diagnostics: the per-chain terms of the tracked state, for rn_k_diag_reduce.
 // The scalar epilogue (b, w, v, rHat, the lag loop with its termination rule, ess) runs on the host in rn_runtime.cpp.
 #ifndef RN_DIAG_CUH
 #define RN_DIAG_CUH
@@ -82,4 +84,107 @@ RN_GLOBAL void rn_k_diag_reduce(const double* RN_RESTRICT in, int C, const doubl
 }
 
 #endif
+
+// Trace.thin(thin).diagnostics accumulated while sampling (rn_sampler_track_diagnostics): no sample block is kept.  Every
+// quantity of the reference is a sum in iteration order that can be carried from one draw to the next -- the chain's sum
+// (Trace.scala:65-67) and, per lag, the variogram sum of (x_t - x_{t-lag})^2 (:112-120) -- and the ESS loop only adds lags
+// 1..99 (`lag < 100`, :106), so a (parameter, chain) pair keeps the last 99 kept draws and 99 variogram accumulators.  The
+// chain variance, a two-pass form around the final mean in the reference (:75-81), is carried as Welford mean and M2.
+// State, RN_DIAG_FIELDS doubles per pair, field-major with the chain fastest: state[(f * n + i) * C + c];
+//   f = 0 sum, 1 Welford mean, 2 Welford M2, 3 + (t % 99) kept draw t of the ring, 3 + 99 + lag - 1 variogram(lag).
+#define RN_DIAG_LAGS 99
+#define RN_DIAG_FIELDS (3 + 2 * RN_DIAG_LAGS)
+#define RN_DIAG_GROUP 9  // lags updated together: 2 shared-memory loads per 9 FMAs (RN_DIAG_LAGS % RN_DIAG_GROUP == 0)
+#ifdef RN_HOST_EMULATION
+static thread_local double* rn_diag_accum_smem;  // the emulation driver's buffer, (RN_DIAG_LAGS + sub) * blockDim.x doubles
+#define RN_DIAG_ACCUM_SMEM rn_diag_accum_smem
+#else
+#define RN_DIAG_ACCUM_SMEM rn_diag_smem
+#endif
+
+// One thread per (chain, parameter): grid = (ceil(C / blockDim.x), n).  s: one sampling launch's draws, [k][n][C]; the
+// launch keeps its draws j0, j0 + thin, .. (m of them), which are kept draws T0 .. T0 + m - 1 of the tracked run.  The
+// thread's column of dynamic shared memory holds rows x[0..99) = kept draws T - 99 .. T - 1 (the ring) and x[99..99+sub) =
+// up to `sub` new draws; per stage every accumulator is loaded once, takes its new terms in increasing t, and is stored
+// once.  The order of every sum is the reference's whatever the launches were, so any split of a run into rn_sampler_run
+// calls gives the same bits.  No warp primitive or barrier: each thread reads and writes only its own column.
+RN_GLOBAL void rn_k_diag_accum(const double* RN_RESTRICT s, int n, int C, int j0, int thin, int m, long long T0, int sub,
+                               double* RN_RESTRICT state) {
+  const int i = blockIdx.y, c = blockIdx.x * blockDim.x + threadIdx.x, B = blockDim.x;
+  if (c >= C) return;
+  const size_t P = (size_t)n * C, at = (size_t)i * C + c;
+  double* st = state + at;
+  double* x = RN_DIAG_ACCUM_SMEM + threadIdx.x;
+#define RN_DIAG_ROW(r) x[(size_t)(r) * B]
+  long long T = T0;
+  for (int r = 0; r < RN_DIAG_LAGS; r++) {  // kept draws of negative index are never read as a term
+    const long long t = T - RN_DIAG_LAGS + r;
+    RN_DIAG_ROW(r) = t >= 0 ? st[(size_t)(3 + t % RN_DIAG_LAGS) * P] : 0.0;
+  }
+  double sum = st[0], mean = st[P], m2 = st[2 * P];
+  for (int r0 = 0; r0 < m; r0 += sub) {
+    const int k = (m - r0) < sub ? (m - r0) : sub;
+    for (int r = 0; r < k; r++) {
+      const double v = s[(size_t)(j0 + (size_t)(r0 + r) * thin) * P + at];
+      RN_DIAG_ROW(RN_DIAG_LAGS + r) = v;
+      sum += v;
+      const double d = v - mean;  // VarianceEstimator-style Welford update, count = kept index + 1
+      mean += d / (double)(T + r + 1);
+      m2 += d * (v - mean);
+    }
+    for (int l0 = 1; l0 <= RN_DIAG_LAGS; l0 += RN_DIAG_GROUP) {
+      double acc[RN_DIAG_GROUP], w[RN_DIAG_GROUP];  // w[g] = x_{t - l0 - g}, slid along t
+      RN_UNROLL
+      for (int g = 0; g < RN_DIAG_GROUP; g++) {
+        acc[g] = st[(size_t)(3 + RN_DIAG_LAGS + l0 + g - 1) * P];
+        w[g] = RN_DIAG_ROW(RN_DIAG_LAGS - l0 - g);
+      }
+      for (int r = 0; r < k; r++) {
+        const double xt = RN_DIAG_ROW(RN_DIAG_LAGS + r);
+        const long long t = T + r;
+        RN_UNROLL
+        for (int g = 0; g < RN_DIAG_GROUP; g++)
+          if (t >= l0 + g) {
+            const double d = xt - w[g];
+            acc[g] += d * d;
+          }
+        RN_UNROLL
+        for (int g = RN_DIAG_GROUP - 1; g > 0; g--) w[g] = w[g - 1];
+        w[0] = RN_DIAG_ROW(RN_DIAG_LAGS + r + 1 - l0);
+      }
+      RN_UNROLL
+      for (int g = 0; g < RN_DIAG_GROUP; g++) st[(size_t)(3 + RN_DIAG_LAGS + l0 + g - 1) * P] = acc[g];
+    }
+    for (int r = 0; r < RN_DIAG_LAGS; r++) RN_DIAG_ROW(r) = RN_DIAG_ROW(r + k);  // the newest 99 rows become the ring
+    T += k;
+  }
+  for (int r = RN_DIAG_LAGS - (m < RN_DIAG_LAGS ? m : RN_DIAG_LAGS); r < RN_DIAG_LAGS; r++) {
+    const long long t = T - RN_DIAG_LAGS + r;
+    if (t >= 0) st[(size_t)(3 + t % RN_DIAG_LAGS) * P] = RN_DIAG_ROW(r);
+  }
+  st[0] = sum;
+  st[P] = mean;
+  st[2 * P] = m2;
+#undef RN_DIAG_ROW
+}
+
+// The per-chain terms of Trace.diagnostics from the tracked state of T kept draws, quantity q = 0 mean (sum / T), 1 variance
+// (M2 / (T - 1)), 1 + lag variogram(lag) / (T - lag) for lag = 1..L -- rn_k_diag_chain's quantity order -- for the quantities
+// q0 .. q0 + nq - 1, so that rn_k_diag_reduce sums them over chains: out[((q - q0) * n + i) * C + c].  One thread per
+// (chain, parameter): grid = (ceil(C / 128), n).
+RN_GLOBAL void rn_k_diag_terms(const double* RN_RESTRICT state, int n, int C, long long T, int L, int q0, int nq, double* RN_RESTRICT out) {
+  const int i = blockIdx.y, c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const size_t P = (size_t)n * C, at = (size_t)i * C + c;
+  for (int q = q0; q < q0 + nq && q <= 1 + L; q++) {
+    double v;
+    if (q == 0)
+      v = state[at] / (double)T;
+    else if (q == 1)
+      v = state[2 * P + at] / (double)(T - 1);
+    else
+      v = state[(size_t)(3 + RN_DIAG_LAGS + q - 2) * P + at] / (double)(T - (q - 1));
+    out[(size_t)(q - q0) * P + at] = v;
+  }
+}
 #endif  // RN_DIAG_CUH

@@ -187,6 +187,7 @@ struct Kernel {
   CUmodule mod = nullptr;
   CUfunction k_init = nullptr, k_iter = nullptr, k_warmup = nullptr, k_density = nullptr, k_transpose = nullptr, k_pool_reduce = nullptr,
              k_pool_apply = nullptr, k_diag_chain = nullptr, k_diag_reduce = nullptr, k_step_pool = nullptr,
+             k_diag_accum = nullptr, k_diag_terms = nullptr,
              k_pool_reduce_dense = nullptr, k_pool_factor = nullptr, k_pool_apply_dense = nullptr;
   const Program* prog = nullptr;
   int backend = 0;            // 0 thread per chain, 1 warp per chain
@@ -539,6 +540,8 @@ static int load_kernel(const Api* A, rn_model* m, Kernel* K) {
   CU(A->cuModuleGetFunction(&K->k_pool_apply, K->mod, "rn_k_pool_apply"));
   CU(A->cuModuleGetFunction(&K->k_diag_chain, K->mod, "rn_k_diag_chain"));
   CU(A->cuModuleGetFunction(&K->k_diag_reduce, K->mod, "rn_k_diag_reduce"));
+  CU(A->cuModuleGetFunction(&K->k_diag_accum, K->mod, "rn_k_diag_accum"));
+  CU(A->cuModuleGetFunction(&K->k_diag_terms, K->mod, "rn_k_diag_terms"));
   if (K->step_pool) CU(A->cuModuleGetFunction(&K->k_step_pool, K->mod, "rn_k_step_pool"));
   if (K->mass_pool) {
     CU(A->cuModuleGetFunction(&K->k_pool_reduce_dense, K->mod, "rn_k_pool_reduce_dense"));
@@ -1024,6 +1027,16 @@ struct rn_sampler {
   std::vector<std::pair<CUevent, CUevent>> allreduce_events;
   double sampling_ms = 0.0;
   int64_t sampling_iterations = 0;
+  // Trace.thin(thin).diagnostics tracked while sampling (rn_sampler_track_diagnostics, rn_diag.cuh): the per-pair state, a
+  // scratch for one launch's draws when rn_sampler_run gets no sample block, and event pairs around the accumulation
+  // launches, whose device time is taken out of sampling_ms
+  bool track = false;
+  int track_thin = 1;
+  int64_t track_seen = 0, track_kept = 0;  // sampling draws since the track call, and how many of them were kept
+  CUdeviceptr d_track = 0, d_track_draws = 0, d_track_terms = 0, d_track_sums = 0;  // state, one launch's draws, finish scratch
+  size_t track_draws_bytes = 0;
+  std::vector<std::pair<CUevent, CUevent>> track_events;  // not yet folded into track_ms
+  double track_ms = 0.0;
 };
 
 namespace {
@@ -1327,14 +1340,14 @@ int rn_sampler_read_trace(rn_sampler* s, double* out /*[chains][iters][4]*/) {
 }
 
 // in-place ncclAllReduce(sum) of `count` elements on the sampler's stream over the attached communicator (no-op without one
-// or with one rank); counted, and timed by event pairs, for rn_sampler_comm_stats
-static int comm_allreduce(const Api* A, rn_sampler* s, CUdeviceptr buf, size_t count, int nccl_type) {
+// or with one rank); the warmup's calls are counted, and timed by event pairs, for rn_sampler_comm_stats
+static int comm_allreduce(const Api* A, rn_sampler* s, CUdeviceptr buf, size_t count, int nccl_type, bool warmup = true) {
   if (!s->comm || s->comm->world <= 1) return RN_OK;
   std::string why;
   const Nccl* N = nccl(&why);
   if (!N) return fail(RN_E_NCCL, why);
   CUevent e0 = nullptr, e1 = nullptr;
-  if (s->allreduce_events.size() < 4096) {  // (pooled steps: one call per warmup iteration)
+  if (warmup && s->allreduce_events.size() < 4096) {  // (pooled steps: one call per warmup iteration)
     CU(A->cuEventCreate(&e0, 0));
     CU(A->cuEventCreate(&e1, 0));
     CU(A->cuEventRecord(e0, s->stream));
@@ -1345,7 +1358,7 @@ static int comm_allreduce(const Api* A, rn_sampler* s, CUdeviceptr buf, size_t c
     s->allreduce_events.push_back({e0, e1});
   }
   if (r != 0) return fail(RN_E_NCCL, std::string("ncclAllReduce: ") + (N->GetErrorString ? N->GetErrorString(r) : "?"));
-  s->allreduce_calls++;
+  if (warmup) s->allreduce_calls++;
   return RN_OK;
 }
 
@@ -1424,6 +1437,52 @@ static int step_pool_apply(const Api* A, rn_sampler* s, int slot, int count, int
   return RN_OK;
 }
 
+// rn_k_diag_accum over the `k` draws one sampling launch wrote at `draws` ([k][n][chains]): the draws whose index since the
+// track call is a multiple of the thin are kept.  Bracketed by an event pair so that rn_chain_stats' times exclude it.
+static const int kTrackSub = 99;      // new draws staged per pass: (99 + 99) rows * 64 threads * 8 bytes = 99 KB of shared memory
+static const int kTrackThreads = 64;
+static const int kTermRows = 8;       // per-chain terms of the finish computed (and reduced) this many quantities at a time
+// fold the accumulation event pairs that have completed into track_ms and release them (all of them when the stream is idle),
+// so that the pairs in flight stay bounded by the launch queue
+static int fold_track_events(const Api* A, rn_sampler* s) {
+  size_t done = 0;
+  for (; done < s->track_events.size(); done++) {
+    float ms = 0.f;
+    const CUresult r = A->cuEventElapsedTime(&ms, s->track_events[done].first, s->track_events[done].second);
+    if (r == 600 /*CUDA_ERROR_NOT_READY*/) break;
+    if (r != 0) return cufail(A, r, "cuEventElapsedTime");
+    s->track_ms += (double)ms;
+    A->cuEventDestroy(s->track_events[done].first);
+    A->cuEventDestroy(s->track_events[done].second);
+  }
+  s->track_events.erase(s->track_events.begin(), s->track_events.begin() + (std::ptrdiff_t)done);
+  return RN_OK;
+}
+static int track_accumulate(const Api* A, rn_sampler* s, CUdeviceptr draws, int k) {
+  const int64_t g0 = s->track_seen, thin = s->track_thin;
+  const int j0 = (int)((thin - g0 % thin) % thin);
+  const int m = j0 < k ? (k - 1 - j0) / (int)thin + 1 : 0;
+  s->track_seen += k;
+  if (m == 0) return RN_OK;
+  int rc = fold_track_events(A, s);
+  if (rc) return rc;
+  CUevent e0 = nullptr, e1 = nullptr;
+  CU(A->cuEventCreate(&e0, 0));
+  CU(A->cuEventCreate(&e1, 0));
+  s->track_events.push_back({e0, e1});
+  CU(A->cuEventRecord(e0, s->stream));
+  int n = (int)s->m->n_params, C = s->chains, j0_ = j0, thin_ = (int)thin, m_ = m, sub = std::min(kTrackSub, m);
+  long long T0 = (long long)s->track_kept;
+  CUdeviceptr st = s->d_track;
+  void* params[] = {&draws, &n, &C, &j0_, &thin_, &m_, &T0, &sub, &st};
+  const unsigned smem = (unsigned)((99 + sub) * kTrackThreads * 8);
+  CU(A->cuLaunchKernel(s->K->k_diag_accum, (unsigned)((C + kTrackThreads - 1) / kTrackThreads), (unsigned)n, 1, kTrackThreads, 1, 1, smem,
+                       s->stream, params, nullptr));
+  CU(A->cuEventRecord(e1, s->stream));
+  s->track_kept += m;
+  return RN_OK;
+}
+
 static int run_phase(const Api* A, rn_sampler* s, int phase, int iterations, double* d_samples, int chain_begin = 0,
                      int chain_end = -1) {
   if (chain_end < 0) chain_end = s->chains;
@@ -1473,6 +1532,18 @@ static int run_phase(const Api* A, rn_sampler* s, int phase, int iterations, dou
     a.win_j = s->win_j;
     a.est_samples = s->est_samples;
     a.samples = (phase == 1 && d_samples) ? d_samples + (size_t)done * s->m->n_params * (size_t)s->chains : nullptr;
+    const bool track = phase == 1 && s->track;
+    if (track && !d_samples) {  // the launch's draws go to the tracker's scratch (grown to the largest launch)
+      const size_t need = (size_t)k * s->m->n_params * (size_t)s->chains * 8;
+      if (s->track_draws_bytes < need) {
+        if (s->d_track_draws) A->cuMemFree(s->d_track_draws);
+        s->d_track_draws = 0;
+        s->track_draws_bytes = 0;
+        CU(A->cuMemAlloc(&s->d_track_draws, need));
+        s->track_draws_bytes = need;
+      }
+      a.samples = (double*)(uintptr_t)s->d_track_draws;
+    }
     a.trace = s->d_trace ? (double*)(uintptr_t)(s->d_trace + s->trace_pos * 4 * (size_t)s->chains * 8) : nullptr;
     int rc = launch(A, s, phase == 0 ? s->K->k_warmup : s->K->k_iter, tail_begin - chain_begin);
     if (rc) return rc;
@@ -1481,6 +1552,10 @@ static int run_phase(const Api* A, rn_sampler* s, int phase, int iterations, dou
       a.chain_begin = tail_begin;
       a.chain_end = chain_end;
       rc = launch(A, s, phase == 0 ? s->K->k_warmup : s->K->k_iter, chain_end - tail_begin);
+      if (rc) return rc;
+    }
+    if (track) {
+      rc = track_accumulate(A, s, (CUdeviceptr)(uintptr_t)a.samples, k);
       if (rc) return rc;
     }
     if (phase == 0) {
@@ -1553,6 +1628,10 @@ int close_sampling_span(const Api* A, rn_sampler* s) {
   float ms = 0.f;
   CU(A->cuEventElapsedTime(&ms, s->ev_run[0], s->ev_run[1]));
   s->sampling_ms += (double)ms;
+  const int rc = fold_track_events(A, s);  // the tracker's accumulation launches inside the span
+  if (rc) return rc;
+  s->sampling_ms -= s->track_ms;
+  s->track_ms = 0.0;
   s->ev_open = false;
   return RN_OK;
 }
@@ -1674,6 +1753,37 @@ int rn_sampler_stats(rn_sampler* s, rn_chain_stats* stats, double* mass, double*
   return RN_OK;
 }
 
+// RN_DIAG_FIELDS of rn_diag.cuh: sum, Welford mean and M2, a ring of the last 99 kept draws, 99 variogram sums
+static const int RN_DIAG_LAGS = 99, RN_DIAG_STATE_DOUBLES = 3 + 2 * RN_DIAG_LAGS;
+
+// the scalar epilogue of Trace.diagnostics (Trace.scala:60,75-109) for one parameter over m chains of I draws: dev2 = sum of
+// (mean_c - meanMean)^2, var_sum = sum of the chain variances, vg[(lag - 1) * stride] = sum of variogram_c(lag) for lag =
+// 1..L (the lags with a non-empty sum that the ESS loop can reach).  out2 = {rHat, effectiveSampleSize}
+static void diag_epilogue(double m, int64_t I, double dev2, double var_sum, const double* vg, size_t stride, int L, double* out2) {
+  const double nn = (double)I;
+  const double b = (nn / (m - 1)) * dev2;        // Trace.scala:75-77
+  const double w = var_sum / m;                  // :88
+  const double v = (nn - 1) / nn * w + b / nn;   // :90-92
+  const double rHat = std::sqrt(v / w);
+  double acc = 0.0;
+  for (int lag = 1;; lag++) {  // Trace.autocorrelation, :97-109 (tail recursion as a loop)
+    double vt;
+    if (lag <= L)
+      vt = vg[(size_t)(lag - 1) * stride] / m;
+    else if (lag == I)
+      vt = std::nan("");  // variogram: 0.0 / 0
+    else
+      vt = -0.0;          // lag > trace.size: empty sum over a negative count
+    const double pt = 1.0 - (vt / (2.0 * v));
+    if (pt > 0.0 && lag < 100)
+      acc += pt;
+    else
+      break;
+  }
+  out2[0] = rHat;
+  out2[1] = nn * m / (1 + (2 * acc));  // :60
+}
+
 // Trace.diagnostics (core/Trace.scala:11-21,49-121) over a device-resident sample block: per-chain sums and the
 // cross-chain reductions on the device (rn_diag.cuh), the scalar epilogue here.  layout 0: [iterations][n][chains] (what
 // rn_sampler_run writes), 1: [chains][iterations][n] (the caller-facing order).  out: host [n][2] = rHat, ess.
@@ -1730,7 +1840,7 @@ int rn_sampler_diagnostics(rn_sampler* s, const double* d_samples, int iteration
   std::vector<double> sums(n_sums);
   CU(A->cuStreamSynchronize(s->stream));
   CU(A->cuMemcpyDtoH(sums.data(), d_sums, (size_t)n * 8));
-  const double m = (double)C, nn = (double)I;
+  const double m = (double)C;
   std::vector<double> meanMean(n);
   for (int i = 0; i < n; i++) meanMean[i] = sums[i] / m;  // means.sum / m, Trace.scala:73
   CU(A->cuMemcpyHtoD(d_shift, meanMean.data(), (size_t)n * 8));
@@ -1738,29 +1848,105 @@ int rn_sampler_diagnostics(rn_sampler* s, const double* d_samples, int iteration
   if (rc) return rc;
   CU(A->cuStreamSynchronize(s->stream));
   CU(A->cuMemcpyDtoH(sums.data(), d_sums, n_sums * 8));
-  for (int i = 0; i < n; i++) {
-    const double b = (nn / (m - 1)) * sums[(2 + (size_t)L) * n + i];  // Trace.scala:75-77
-    const double w = sums[n + i] / m;                                  // :88
-    const double v = (nn - 1) / nn * w + b / nn;                       // :90-92
-    const double rHat = std::sqrt(v / w);
-    double acc = 0.0;
-    for (int lag = 1;; lag++) {  // Trace.autocorrelation, :97-109 (tail recursion as a loop)
-      double vt;
-      if (lag <= L)
-        vt = sums[(2 + (size_t)(lag - 1)) * n + i] / m;
-      else if (lag == I)
-        vt = std::nan("");  // variogram: 0.0 / 0
-      else
-        vt = -0.0;          // lag > trace.size: empty sum over a negative count
-      const double pt = 1.0 - (vt / (2.0 * v));
-      if (pt > 0.0 && lag < 100)
-        acc += pt;
-      else
-        break;
-    }
-    out[2 * i] = rHat;
-    out[2 * i + 1] = nn * m / (1 + (2 * acc));  // :60
+  for (int i = 0; i < n; i++)
+    diag_epilogue(m, I, sums[(2 + (size_t)L) * n + i], sums[n + i], &sums[2 * (size_t)n + i], n, L, out + 2 * i);
+  return RN_OK;
+}
+
+// Trace.thin(thin).diagnostics from here on, accumulated after every sampling launch (track_accumulate, rn_k_diag_accum)
+int rn_sampler_track_diagnostics(rn_sampler* s, int thin) {
+  if (!s) return fail(RN_E_INVALID, "null sampler");
+  if (thin < 1) return fail(RN_E_INVALID, "thin must be >= 1");
+  std::lock_guard<std::recursive_mutex> model_lock_(s->m->mu);
+  std::string why;
+  const Api* A = api(&why);
+  if (!A) return fail(RN_E_CUDA, why);
+  CU(A->cuCtxSetCurrent(s->m->ctx));
+  const size_t n = s->m->n_params, nC = n * (size_t)s->chains, bytes = (size_t)RN_DIAG_STATE_DOUBLES * nC * 8;
+  if (!s->d_track) {  // the finish allocates nothing, so a rank cannot fail there on memory while the others all-reduce
+    CU(A->cuMemAlloc(&s->d_track, std::max<size_t>(bytes, 8)));
+    CU(A->cuMemAlloc(&s->d_track_terms, (size_t)kTermRows * nC * 8));
+    CU(A->cuMemAlloc(&s->d_track_sums, (5 + n + (2 + (size_t)RN_DIAG_LAGS) * n + n) * 8));
+    CU(A->cuFuncSetAttribute(s->K->k_diag_accum, 8 /*MAX_DYNAMIC_SHARED_SIZE_BYTES*/, (99 + kTrackSub) * kTrackThreads * 8));
   }
+  CU(A->cuMemsetD8Async(s->d_track, 0, bytes, s->stream));
+  s->track = true;
+  s->track_thin = thin;
+  s->track_seen = s->track_kept = 0;
+  return RN_OK;
+}
+
+// Two passes over this rank's chains, each a fixed-order reduction (rn_k_diag_terms, rn_k_diag_reduce) followed by one sum
+// all-reduce over the ranks: {ranks not tracking, ranks whose pass 0 failed on the device, C_r, T_r, T_r^2, sum_c mean_c},
+// then {sum_c (mean_c - meanMean)^2, sum_c var_c, sum_c variogram_c(lag) / (T - lag)}.  A rank's own failures before the
+// first all-reduce are carried by it, and every verdict after it is taken from all-reduced numbers, so all ranks fail
+// together or go on together.  The per-chain terms are made kTermRows quantities at a time in the tracker's scratch.
+int rn_sampler_tracked_diagnostics(rn_sampler* s, double* out) {
+  if (!s || !out) return fail(RN_E_INVALID, "null argument");
+  std::lock_guard<std::recursive_mutex> model_lock_(s->m->mu);
+  std::string why;
+  const Api* A = api(&why);
+  if (!A) return fail(RN_E_CUDA, why);
+  CU(A->cuCtxSetCurrent(s->m->ctx));
+  const size_t n = s->m->n_params, C = (size_t)s->chains;
+  const int64_t T = s->track_kept;
+  const int L = (int)std::max<int64_t>(0, std::min<int64_t>(RN_DIAG_LAGS, T - 1));
+  const size_t nq = 2 + (size_t)L;
+  // a rank that never tracked has no scratch: it takes part in the first all-reduce with a buffer of its own
+  struct Scratch {
+    const Api* A;
+    CUdeviceptr p = 0;
+    ~Scratch() {
+      if (p) A->cuMemFree(p);
+    }
+  } own{A};
+  if (!s->track) CU(A->cuMemAlloc(&own.p, (5 + n) * 8));
+  const CUdeviceptr buf = s->track ? s->d_track_sums : own.p, d_pass1 = buf + (5 + n) * 8, d_shift = d_pass1 + nq * n * 8;
+  int n_ = (int)n, C_ = (int)C, L_ = L;
+  long long T_ = (long long)T;
+  auto terms = [&](int q0, int nrows) -> CUresult {  // per-chain quantities q0 .. q0 + nrows - 1 -> d_track_terms
+    CUdeviceptr st = s->d_track, tp = s->d_track_terms;
+    void* params[] = {&st, &n_, &C_, &T_, &L_, &q0, &nrows, &tp};
+    s->launches++;
+    return A->cuLaunchKernel(s->K->k_diag_terms, (unsigned)((C + 127) / 128), (unsigned)n, 1, 128, 1, 1, 0, s->stream, params, nullptr);
+  };
+  auto reduce = [&](size_t rows, CUdeviceptr shift, CUdeviceptr outp) -> CUresult {  // over the chains of d_track_terms
+    CUdeviceptr in = s->d_track_terms;
+    void* params[] = {&in, &C_, &shift, &outp};
+    s->launches++;
+    return A->cuLaunchKernel(s->K->k_diag_reduce, (unsigned)rows, 1, 1, 256, 1, 1, 0, s->stream, params, nullptr);
+  };
+  bool failed = A->cuMemsetD8Async(buf, 0, (5 + n) * 8, s->stream) != 0;
+  if (s->track && !failed) failed = terms(0, 1) != 0 || reduce(n, 0, buf + 5 * 8) != 0;  // sum of the chain means
+  const double head[5] = {s->track ? 0.0 : 1.0, failed ? 1.0 : 0.0, (double)C, (double)T, (double)T * (double)T};
+  CU(A->cuMemcpyHtoDAsync(buf, head, sizeof(head), s->stream));
+  int rc = comm_allreduce(A, s, buf, 5 + n, 8 /*ncclFloat64*/, false);
+  if (rc) return rc;
+  std::vector<double> h(5 + n + nq * n);
+  CU(A->cuStreamSynchronize(s->stream));
+  CU(A->cuMemcpyDtoH(h.data(), buf, (5 + n) * 8));
+  const double R = (s->comm && s->comm->world > 1) ? (double)s->comm->world : 1.0;
+  if (h[0] > 0) return fail(RN_E_INVALID, "rn_sampler_tracked_diagnostics before rn_sampler_track_diagnostics (on at least one rank)");
+  if (h[1] > 0) return fail(RN_E_CUDA, "tracked diagnostics: a launch of the first pass failed (on at least one rank)");
+  if (h[2] < 2) return fail(RN_E_INVALID, "requirement failed: diagnostics requires multiple chains (Trace.scala:12)");
+  if (R * h[4] != h[3] * h[3]) return fail(RN_E_INVALID, "tracked diagnostics: the ranks kept different numbers of draws");
+  if (T < 2) return fail(RN_E_INVALID, "tracked diagnostics need at least 2 kept draws");
+  const double m = h[2];
+  std::vector<double> meanMean(n);
+  for (size_t i = 0; i < n; i++) meanMean[i] = h[5 + i] / m;  // means.sum / m, Trace.scala:73
+  CU(A->cuMemcpyHtoDAsync(d_shift, meanMean.data(), n * 8, s->stream));
+  CU(reduce(n, d_shift, d_pass1));  // sum_c (mean_c - meanMean)^2, over the means pass 0 left in the scratch
+  for (int q0 = 1; q0 < (int)nq; q0 += kTermRows) {  // variances, variograms
+    const int rows = std::min<int>(kTermRows, (int)nq - q0);
+    CU(terms(q0, rows));
+    CU(reduce((size_t)rows * n, 0, d_pass1 + (size_t)q0 * n * 8));
+  }
+  rc = comm_allreduce(A, s, d_pass1, nq * n, 8 /*ncclFloat64*/, false);
+  if (rc) return rc;
+  CU(A->cuStreamSynchronize(s->stream));
+  CU(A->cuMemcpyDtoH(h.data() + 5 + n, d_pass1, nq * n * 8));
+  const double* p1 = h.data() + 5 + n;
+  for (size_t i = 0; i < n; i++) diag_epilogue(m, T, p1[i], p1[n + i], &p1[2 * n + i], n, L, out + 2 * i);
   return RN_OK;
 }
 
@@ -1812,6 +1998,14 @@ void rn_sampler_destroy(rn_sampler* s) {
       }
     }
     if (s->d_trace) A->cuMemFree(s->d_trace);
+    if (s->d_track) A->cuMemFree(s->d_track);
+    if (s->d_track_terms) A->cuMemFree(s->d_track_terms);
+    if (s->d_track_sums) A->cuMemFree(s->d_track_sums);
+    if (s->d_track_draws) A->cuMemFree(s->d_track_draws);
+    for (auto& pr : s->track_events) {
+      A->cuEventDestroy(pr.first);
+      A->cuEventDestroy(pr.second);
+    }
     for (CUevent e : s->ev_run)
       if (e) A->cuEventDestroy(e);
     for (auto& pr : s->allreduce_events) {

@@ -7,7 +7,9 @@ chain block `chain_block(total, r, world)` with the same per-chain seeds a singl
 rank-local until gathered.  The only exchange step is optional and warmup-only: pooling mass-matrix window statistics
 over all chains of all ranks (RN_ADAPT_POOLED) -- two sum all-reduces per window of the chains' Welford statistics: first
 {chains, sum of the chains' window means} (n+1 doubles), then sum of M2_c + L (mean_c - pooled mean)^2 (n doubles), or
-with the dense tuner the n^2 sums of C2_c[j][k] + L d_c[j] d_c[k] (`combine_welford_dense`).
+with the dense tuner the n^2 sums of C2_c[j][k] + L d_c[j] d_c[k] (`combine_welford_dense`).  Tracked diagnostics
+(rn_sampler_tracked_diagnostics) are the other collective, on demand: two all-reduces of the same shape
+(`combine_diagnostics`).
 
 torch.distributed is used purely as plumbing (NCCL on GPUs, gloo in the CPU tests).
 """
@@ -57,6 +59,71 @@ def combine_welford_dense(n, mean, cov):
     k = mean.shape[0]
     d = mean - mean.sum(axis=0) / k
     return (cov + n * d[:, :, None] * d[:, None, :]).sum(axis=0) / (k * n)
+
+
+DIAG_LAGS = 99  # variogram lags the ESS loop of Trace.diagnostics can add (Trace.scala:106)
+
+
+def diagnostics_pass0(kept, sums):
+    """Host mirror of pass 0 of rn_sampler_tracked_diagnostics on one rank: kept draws T_r per chain and the chains' running
+    sums [C_r][n] -> the vector that is all-reduced, [0 (not tracking), 0 (out of memory), C_r, T_r, T_r^2, sum_c mean_c]"""
+    sums = np.asarray(sums, dtype=np.float64)
+    return np.concatenate([[0.0, 0.0, sums.shape[0], kept, float(kept) * float(kept)], (sums / kept).sum(axis=0)])
+
+
+def equal_kept_counts(world, pass0_total):
+    """the all-reduced verdict that every rank kept the same number of draws: R * sum T_r^2 == (sum T_r)^2, exact in fp64"""
+    return world * pass0_total[4] == pass0_total[3] * pass0_total[3]
+
+
+def diagnostics_pass1(kept, sums, m2, vg, pass0_total):
+    """pass 1 on one rank around the pooled mean of pass 0: [sum_c (mean_c - meanMean)^2, sum_c M2_c / (T - 1),
+    sum_c vg_c(lag) / (T - lag) for lag = 1..L], L = min(99, T - 1); vg: [C_r][99][n] variogram sums"""
+    sums, m2, vg = (np.asarray(a, dtype=np.float64) for a in (sums, m2, vg))
+    L = min(DIAG_LAGS, kept - 1)
+    mm = pass0_total[5:] / pass0_total[2]
+    lags = np.arange(1, L + 1, dtype=np.float64)[None, :, None]
+    return np.concatenate([((sums / kept - mm) ** 2).sum(axis=0), (m2 / (kept - 1)).sum(axis=0),
+                           (vg[:, :L, :] / (kept - lags)).sum(axis=0).reshape(-1)])
+
+
+def diagnostics_epilogue(chains, kept, dev2, var_sum, vg_sum):
+    """Trace.scala:60,75-109 for one parameter (rn_runtime.cpp: diag_epilogue): vg_sum[lag - 1] for lag = 1..L"""
+    m, nn, L = float(chains), float(kept), len(vg_sum)
+    b = (nn / (m - 1)) * dev2
+    w = var_sum / m
+    v = (nn - 1) / nn * w + b / nn
+    acc, lag = 0.0, 1
+    while True:
+        vt = vg_sum[lag - 1] / m if lag <= L else (np.nan if lag == kept else -0.0)
+        pt = 1.0 - (vt / (2.0 * v))
+        if not (pt > 0.0 and lag < 100):
+            break
+        acc, lag = acc + pt, lag + 1
+    return np.sqrt(v / w), nn * m / (1 + (2 * acc))
+
+
+def diagnostics_finish(kept, pass0_total, pass1_total):
+    """[n][2] = (rHat, effectiveSampleSize) from the two all-reduced vectors"""
+    n = len(pass0_total) - 5
+    p1 = np.asarray(pass1_total).reshape(-1, n)
+    return np.array([diagnostics_epilogue(pass0_total[2], kept, p1[0, i], p1[1, i], p1[2:, i]) for i in range(n)])
+
+
+def combine_diagnostics(blocks):
+    """Host mirror of rn_sampler_tracked_diagnostics over ranks: blocks[r] = (T_r, sums [C_r][n], M2 [C_r][n], variogram
+    sums [C_r][99][n]) of rank r's chains; the two all-reduces are sums in rank order.  Raises ValueError where the library
+    returns RN_E_INVALID."""
+    p0 = sum(diagnostics_pass0(b[0], b[1]) for b in blocks)
+    if p0[2] < 2:
+        raise ValueError("requirement failed: diagnostics requires multiple chains (Trace.scala:12)")
+    if not equal_kept_counts(len(blocks), p0):
+        raise ValueError("the ranks kept different numbers of draws")
+    kept = blocks[0][0]
+    if kept < 2:
+        raise ValueError("at least 2 kept draws")
+    p1 = sum(diagnostics_pass1(b[0], b[1], b[2], b[3], p0) for b in blocks)
+    return diagnostics_finish(kept, p0, p1)
 
 
 def allreduce_window_stats(stats, group=None):

@@ -56,5 +56,13 @@ public final class Native {
   /** rn_optimize: Optimizer.lbfgs for a batch of starts; x0 == null: every start at 0 (the reference's start) */
   public static native void optimize(long handle, double[] x0, int starts, int m, double eps, int maxEvals, double[] x, int[] info);
 
+  /** rn_sampler_track_diagnostics: Trace.thin(thin).diagnostics accumulated on the device over the sampler's following
+   *  sampling iterations; sampler is an rn_sampler handle of the staged API */
+  public static native void samplerTrackDiagnostics(long sampler, int thin);
+
+  /** rn_sampler_tracked_diagnostics: out [n][2] = rHat, effectiveSampleSize over the tracked draws of every chain (every rank
+   *  of an attached communicator calls it) */
+  public static native void samplerTrackedDiagnostics(long sampler, double[] out);
+
   public static native String lastError();
 }

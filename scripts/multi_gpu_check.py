@@ -1,6 +1,6 @@
 """torchrun --nproc-per-node N scripts/multi_gpu_check.py : chains sharded over ranks reproduce the single-GPU run bit
 for bit (no collective on the sampling path), and RN_ADAPT_POOLED all-reduces window statistics over NCCL so that every
-rank ends warmup with the same shared mass matrix."""
+rank ends warmup with the same shared mass matrix; tracked diagnostics cover every chain of every rank, identically on all."""
 import os
 import sys
 
@@ -61,6 +61,37 @@ if rank == 0:
     assert np.array_equal(full, ref.chains), "pooled steps: sharded run differs from the single-GPU run"
     print("pooled step sizes: %d ranks x %d chains == 1 rank x %d chains bit for bit; %d all-reduce calls"
           % (world, total // world, total, calls))
+
+# tracked diagnostics over NCCL: Trace.diagnostics of every chain of every rank, the same numbers on every rank
+from oracle.rainier_py.diagnostics import trace_diagnostics  # noqa: E402
+cfgt = api.SamplerConfig(iterations=300, warmupIterations=300)
+s = api.CudaSampler(model, cfgt, seeds=mine)
+s.set_comm(comm)
+d = torch.empty((300, model.nVars, len(mine)), dtype=torch.float64, device="cuda")
+s.warmup(-1)
+s.track_diagnostics(1)
+s.run(120, d.data_ptr())
+s.run(180, d[120:].data_ptr())
+got = s.tracked_diagnostics()
+s.close()
+g = torch.tensor(got, device="cuda")
+gathered = [torch.empty_like(g) for _ in range(world)]
+dist.all_gather(gathered, g)
+assert all(torch.equal(x, gathered[0]) for x in gathered), "ranks disagree on the tracked diagnostics"
+full = rdist.gather_samples(d.permute(2, 0, 1).contiguous().cpu().numpy(), total)
+if rank == 0:
+    one = api.CudaSampler(model, cfgt, seeds=seeds)
+    one.warmup(-1)
+    one.track_diagnostics(1)
+    one.run(300)
+    single = one.tracked_diagnostics()
+    one.close()
+    rel = lambda a, b: float(np.max(np.abs(a - b) / np.maximum(np.abs(b), 1e-12)))
+    assert rel(got, single) < 1e-12, (got, single)
+    ref = np.array(trace_diagnostics(full))
+    assert rel(got, ref) < 1e-9, (got, ref)
+    print("tracked diagnostics: identical on all %d ranks; vs one process %.2g, vs the restatement %.2g"
+          % (world, rel(got, single), rel(got, ref)))
 
 # BASELINE.json configs[3]: eight schools, DefaultConfig (EHMC + DualAvg + diagonal mass), 8192 chains over the ranks,
 # warmup with the pooled mass-matrix all-reduce (NCCL over NVLink); device-resident, timed on the device, max over ranks
