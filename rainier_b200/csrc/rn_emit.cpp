@@ -404,6 +404,14 @@ struct Emitter {
     return true;
   }
 
+  // the literal +0.0: accumulating it is an exact no-op and is not emitted.  Every accumulator starts at +0.0 and only ever
+  // has values added to it; a round-to-nearest sum is -0.0 only when both operands are, so an accumulator never holds -0.0
+  // and x + (+0.0) == x bit for bit (NaN stays NaN).  (A -0.0 term is still added: that addition is what makes it +0.0.)
+  bool is_pos_zero(int id) const {
+    const Node& n = P.nodes[id];
+    return n.kind == K_CONST && n.value == 0.0 && !std::signbit(n.value);
+  }
+
   std::string val(int id) const {
     if (!name_override.empty()) {
       auto it = name_override.find(id);
@@ -609,7 +617,8 @@ struct Emitter {
             [&](int slot) { return "acc[" + std::to_string(slot) + "]"; }, false, 0);
         os << "  }\n";
       } else {
-        for (const AccStmt& a : T.row_acc) os << "  acc[" << a.slot << "] += " << val(a.node) << ";\n";
+        for (const AccStmt& a : T.row_acc)
+          if (!is_pos_zero(a.node)) os << "  acc[" << a.slot << "] += " << val(a.node) << ";\n";
       }
     }
     os << "  dens = acc[0];\n";
@@ -1750,7 +1759,8 @@ struct Emitter {
         os << "    }\n  }\n";
       } else {
         os << "  if (lane == 0) {\n";  // counted once by the reduction below
-        for (const AccStmt& a : T.row_acc) os << "    " << acc_ref(a.slot) << " += " << val(a.node) << ";\n";
+        for (const AccStmt& a : T.row_acc)
+          if (!is_pos_zero(a.node)) os << "    " << acc_ref(a.slot) << " += " << val(a.node) << ";\n";
         os << "  }\n";
       }
     }
@@ -1879,6 +1889,7 @@ std::string emit_source(const Program& P, const EmitOptions& opt) {
   if (opt.step_pool) os << "#define RN_STEP_POOL 1\n";
   if (opt.mass_pool) os << "#define RN_MASS_POOL 1\n";
   if (opt.fast_math) os << "#define RN_FAST_MATH 1\n";
+  if (opt.backend == 0) os << "#define RN_TS_RESTORE " << (opt.tpc_restore ? 1 : 0) << "\n";
   if (opt.backend == 1) {
     os << "#define RN_WPC_K " << std::max(1, opt.wpc_k) << "\n";
     os << "#define RN_TMA_STAGES " << opt.tma_stages << "\n";

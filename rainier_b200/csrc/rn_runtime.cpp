@@ -181,6 +181,19 @@ static unsigned tpc_block_for(size_t chains, unsigned sms) {
   if (const char* e = getenv("RN_BLOCK")) block = std::max(32u, std::min(128u, (unsigned)atoi(e) & ~31u));
   return block;
 }
+// Whether the thread-per-chain sampler keeps its iteration's restore point (q, gradient, potential: 2n + 1 doubles per thread) in
+// shared memory (rn_sampler.cuh: RN_TS_RESTORE) -- only where that costs no occupancy.  Threads per SM are counted for CTAs of
+// `block` threads (0: not fixed; 128, the largest) with `without` / `with` bytes of shared memory per thread, 228 KB per SM and
+// 1 KB reserved per CTA; the slots go on chip when an SM still holds as many threads as the register file allows at 128
+// registers per thread (512; models with n > 16 take more registers and so fewer threads).  Every CTA the module may be launched
+// with must fit as well (load_kernel opts in to 128 threads' worth).  The funnel and the other n = 10 identity / static-matrix
+// HMC configurations keep 512 threads per SM with the slots; EHMC with an adapted mass matrix at n = 10 and large n keep the
+// restore point in `params`.
+static bool tpc_restore_on_chip(unsigned without, unsigned with, unsigned block) {
+  if (block == 0) block = 128u;
+  auto threads_per_sm = [block](unsigned per_thread) { return std::min(32u, (228u * 1024u) / (per_thread * block + 1024u)) * block; };
+  return with * 128u <= 227u * 1024u && threads_per_sm(with) >= std::min(512u, threads_per_sm(without));
+}
 struct Kernel {
   std::string source;
   std::vector<char> cubin;
@@ -202,7 +215,7 @@ struct Kernel {
   bool mma = false;           // backend 1: chain-batched DMMA path compiled in (tile_doubles = its shared doubles)
   int mma_chains = 8;         //            chains per CTA on that path (8 or 16)
   // backend 0: bytes of dynamic shared memory per THREAD (rn_sampler.cuh: momentum, diagonal mass, EHMC snapshot momentum,
-  // Stats counters live there instead of in registers) -- must mirror RN_TS_DOUBLES / RN_TS_INTS
+  // Stats counters and, where it fits, the restore point live there instead of in registers) -- must mirror RN_TS_DOUBLES / RN_TS_INTS
   unsigned tpc_smem_per_thread = 0;
   unsigned smem_bytes() const {  // dynamic shared memory of one CTA: per-warp slices | 128B pad | stages | mbarriers
     size_t d = (size_t)warps_per_cta * wpc_smem_doubles;
@@ -339,7 +352,9 @@ static int get_kernel(rn_model* m, const rn_config* cfg, Kernel** out, std::stri
   if (eo.backend == 0) {  // rn_sampler.cuh: RN_TS_DOUBLES * 8 + RN_TS_INTS * 4
     const unsigned n = P->n_params;
     const unsigned doubles = (n + 1) + (key.mass_max >= 1 ? n : 0) + (key.ehmc ? n : 0) + 5 + 4;
-    K->tpc_smem_per_thread = doubles * 8 + 10 * 4;
+    const unsigned bytes = doubles * 8 + 10 * 4, with_restore = bytes + (2 * n + 1) * 8;
+    eo.tpc_restore = tpc_restore_on_chip(bytes, with_restore, (unsigned)key.block);
+    K->tpc_smem_per_thread = eo.tpc_restore ? with_restore : bytes;
     if ((size_t)K->tpc_smem_per_thread * 32 > 227 * 1024 - 1024)
       return fail(RN_E_UNSUPPORTED, "thread-per-chain shape: the chain's shared-memory state does not fit; use RN_BACKEND_WARP");
   }

@@ -43,12 +43,23 @@
 #else
 #define RN_TS_NSNAP 0
 #endif
+// RN_TS_RESTORE (set by the emitter): the iteration's restore point has slots here -- the runtime allots them only where their
+// 2n + 1 doubles per thread cost no CTA per SM (rn_runtime.cpp: tpc_restore_on_chip); elsewhere it stays in `params` / `grad`
+#ifndef RN_TS_RESTORE
+#define RN_TS_RESTORE 0
+#endif
+#if RN_TS_RESTORE
+#define RN_TS_NREST (2 * RN_N + 1)
+#else
+#define RN_TS_NREST 0
+#endif
 #define RN_TS_P 0                                        /* momentum, RN_N + 1 slots (+1: scratch of the polar method) */
 #define RN_TS_MASS (RN_N + 1)                            /* diagonal mass matrix (variances) */
 #define RN_TS_SNAP (RN_TS_MASS + RN_TS_NMASS)            /* momentum of the EHMC snapshot */
 #define RN_TS_STAT (RN_TS_SNAP + RN_TS_NSNAP)            /* e_mean, e_raw, trans2, grads (i64), steps (i64) */
 #define RN_TS_HOT (RN_TS_STAT + 5)                       /* rng.seed (i64), rng.nng, prevH, startH: parked across the leapfrog */
-#define RN_TS_DOUBLES (RN_TS_HOT + 4)
+#define RN_TS_REST (RN_TS_HOT + 4)                       /* restore point: q, gradient, potential at startIteration */
+#define RN_TS_DOUBLES (RN_TS_REST + RN_TS_NREST)
 #define RN_TS_INTS 10                                    /* iters, accepted, e_n, ring_i[3], ring_full[3], rng.have */
 struct RnTs {
   double* d;
@@ -106,6 +117,9 @@ RN_DEVICE RnTs rn_ts_get() {
 #define RN_ST_RING_FULL(r) RN_TSI(6 + (r))
 #define RN_TS_PREV_H RN_TSD(RN_TS_HOT + 2)
 #define RN_TS_START_H RN_TSD(RN_TS_HOT + 3)
+#define RN_REST_Q(i) RN_TSD(RN_TS_REST + (i))
+#define RN_REST_G(i) RN_TSD(RN_TS_REST + RN_N + (i))
+#define RN_REST_U RN_TSD(RN_TS_REST + 2 * RN_N)
 
 // counters of the iteration in flight (registers; folded into the shared-memory Stats once per iteration)
 struct RnIt {
@@ -516,6 +530,17 @@ RN_GLOBAL void rn_k_init(const RnArgs A) {
 // Driver.collectSamples (PHASE 1, Driver.scala:102-117).  Two entry points of one body so that the sampling kernel
 // carries neither the code nor the registers of the adaptation.
 // =============================================================================================================
+// where the momentum `params` must hold lives while the restore point is on chip (RN_REST_ON_CHIP): already in `params`, in the
+// registers (the final momentum of an accepted proposal), or in the scratch of the normal draws (the momentum drawn for a
+// rejected proposal under the identity mass)
+enum { RN_P_IN_PARAMS = 0, RN_P_IN_REGS = 1, RN_P_IN_Z = 2 };
+RN_DEVICE void rn_store_momentum(const RnArgs& A, int c, const RnTs& T, const RnPQ& s, int where) {
+  (void)s;
+  if (where == RN_P_IN_PARAMS) return;
+  RN_UNROLL
+  for (int i = 0; i < RN_N; i++) RN_AT(A.params, i, c) = where == RN_P_IN_REGS ? RN_P(i) : RN_Z(i);
+}
+
 template <int PHASE>
 RN_DEVICE void rn_iterate(const RnArgs& A) {
   const int c = A.chain_begin + (int)(blockIdx.x * blockDim.x + threadIdx.x);
@@ -533,7 +558,11 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
   S.grads = 0;
   S.steps = 0;
   S.err = 0;
+#if RN_MASS_MAX >= 1
   int kind = A.mass_kind;
+#else
+  constexpr int kind = 0;  // identity only: the momentum stores of the other kinds vanish at compile time
+#endif
   rn_load_mass(A, c, T, kind);
 
   // step size in force: warmup uses the tuner's running value; sampling uses stepSizeTuner.stepSize
@@ -555,14 +584,24 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
   bool havePrevH = false;
 
   // RN_X_KEEP_STATE: the current position, its gradient and potential stay in registers from one iteration to the next -- after an
-  // accepted proposal they ARE the state the next iteration starts from, so only a rejection re-reads them from `params` (which is
-  // written on accept exactly as before: it is what a rejection restores, what isUTurn measures against, and the state the launch
-  // leaves behind).  The drawn momentum reaches `params` only where the reference's copy survives the iteration: on rejection
-  // (from the scratch of the normal draws, intact while the momentum lives in registers under the identity mass).
+  // accepted proposal they ARE the state the next iteration starts from, so only a rejection restores them.  The drawn momentum
+  // reaches `params` only where the reference's copy survives the iteration: on rejection (from the scratch of the normal draws,
+  // intact while the momentum lives in registers under the identity mass).
+  // RN_REST_ON_CHIP: the restore point (q, gradient, potential at startIteration) is kept in this thread's shared-memory slots;
+  // a rejection and isUTurn read it there, and `params` / `grad` are written once, when the launch ends (or, for the momentum,
+  // where a window end makes the next iteration read it).  Otherwise `params` is written on every accepted proposal and is
+  // itself the restore point.  Between launches `params` / `grad` hold the same state either way.
 #ifndef RN_X_KEEP_STATE
 #define RN_X_KEEP_STATE 1 /* with the compile-time CTA size */
 #endif
 #define RN_KEEP_P_LATE (RN_X_KEEP_STATE && RN_X_P_REGS)
+#define RN_REST_ON_CHIP (RN_X_KEEP_STATE && RN_TS_RESTORE)
+#if RN_REST_ON_CHIP
+#define RN_X0(i) RN_REST_Q(i)
+  int p_at = RN_P_IN_PARAMS;
+#else
+#define RN_X0(i) RN_AT(A.params, RN_N + (i), c)
+#endif
   RnPQ s;
 #if RN_X_KEEP_STATE
   RN_UNROLL
@@ -605,6 +644,14 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
 #endif
     s.U = cU;
     RN_TS_START_H = rn_energy(A, c, T, s, kind, cU);  // finishIteration's energy(params), :62
+#if RN_REST_ON_CHIP
+    RN_UNROLL
+    for (int i = 0; i < RN_N; i++) {
+      RN_REST_Q(i) = s.q[i];
+      RN_REST_G(i) = s.g[i];
+    }
+    RN_REST_U = cU;
+#endif
     const double usedStep = stepSize;
 
     // ---------------- sampler.warmup / sampler.run ----------------
@@ -626,7 +673,7 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
         for (;;) {
           double out = 0.0;  // lf.isUTurn(params), LeapFrog.scala:35-47
           RN_UNROLL
-          for (int i = 0; i < RN_N; i++) out += (s.q[i] - RN_AT(A.params, RN_N + i, c)) * RN_P(i);
+          for (int i = 0; i < RN_N; i++) out += (s.q[i] - RN_X0(i)) * RN_P(i);
           const bool uturn = (out != out) ? true : (out < 0);
           if (uturn || !(l < A.max_steps)) break;
           l += 1;
@@ -676,6 +723,9 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
     }
     double eH;
     if (accept) {
+#if RN_REST_ON_CHIP
+      p_at = RN_P_IN_REGS;
+#else
       RN_UNROLL
       for (int i = 0; i < RN_N; i++) {
         RN_AT(A.params, i, c) = RN_P(i);
@@ -683,9 +733,19 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
         RN_AT(A.grad, i, c) = s.g[i];
       }
       RN_AT(A.params, 2 * RN_N, c) = s.U;
+#endif
       eH = endH;
       RN_ST_ACCEPTED += 1;
     } else {
+#if RN_REST_ON_CHIP
+      RN_UNROLL
+      for (int i = 0; i < RN_N; i++) {
+        s.q[i] = RN_REST_Q(i);
+        s.g[i] = RN_REST_G(i);
+      }
+      s.U = RN_REST_U;
+      p_at = (RN_KEEP_P_LATE && kind == 0) ? RN_P_IN_Z : RN_P_IN_PARAMS;  // else stored at startIteration (LeapFrog.scala:55)
+#else
       RN_UNROLL
       for (int i = 0; i < RN_N; i++) s.q[i] = RN_AT(A.params, RN_N + i, c);  // s.q := current position either way
 #if RN_X_KEEP_STATE
@@ -696,6 +756,7 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
         RN_UNROLL
         for (int i = 0; i < RN_N; i++) RN_AT(A.params, i, c) = RN_Z(i);
       }
+#endif
 #endif
       eH = startH;
     }
@@ -801,6 +862,10 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
             win_i = 0;
             win_size = rn_d2i(win_size * A.win_expansion);
             havePrevH = false;  // the next startIteration measures params with the NEW matrix
+#if RN_REST_ON_CHIP
+            rn_store_momentum(A, c, T, s, p_at);  // ... and reads its momentum there
+            p_at = RN_P_IN_PARAMS;
+#endif
             if (A.mass_tuner == 1) {  // DiagonalMassMatrix(variance()), :92-103
               kind = 1;
               RN_UNROLL
@@ -847,6 +912,15 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
     }
   }
 
+#if RN_REST_ON_CHIP
+  rn_store_momentum(A, c, T, s, p_at);  // the state the launch leaves behind
+  RN_UNROLL
+  for (int i = 0; i < RN_N; i++) {
+    RN_AT(A.params, RN_N + i, c) = s.q[i];
+    RN_AT(A.grad, i, c) = s.g[i];
+  }
+  RN_AT(A.params, 2 * RN_N, c) = s.U;
+#endif
   if (PHASE == 0) RN_AT(A.da, 0, c) = stepSize;
 #if RN_ENABLE_EHMC
   if (A.sampler == 1) {
