@@ -313,6 +313,52 @@ void rn_function_destroy(rn_function* f);
 int rn_sample_predict(rn_model* m, const rn_config* cfg, rn_function* f, const int64_t* seeds, int chains, double* predictions,
                       double* mass, rn_chain_stats* stats);
 
+/* ---- posterior-predictive draws: the Generator.get half of Trace.predict ------------------------------------ */
+/* rn_generator_*       <- `chains.flatMap(_.map(fn))` of Trace.predict (rainier-core/.../core/Trace.scala:34-41) with
+ *                         fn = Generator.prepare's closure (core/Generator.scala:59-94): for every posterior draw the
+ *                         generator's requirement values AND its RNG-consuming Generator.get, on the device, for the
+ *                         built-in distributions (Continuous.scala, Discrete.scala), Real values, tuples, Seq/Vec and
+ *                         repeat(k) with a constant k.
+ * rir: a RIR_FLAG_FUNCTION | RIR_FLAG_GENERATOR container (rainier_rir.h): n inputs (the model's parameters), the slots as
+ * the function's outputs, the plan; m_out doubles per draw (rn_generator_noutputs), discrete values as Java Longs stored as
+ * doubles.  device -1: emit/compile only.  Always parity math.
+ * Stream rule: chain c owns rng_states[c] and draws its iterations in order, exactly as the reference's predict over a Trace
+ * holding chain c alone with an RNG in that state; the state after the last draw is written back.  Any split of the
+ * iterations into calls gives the same bits.
+ * Bounded work: every draw of a built-in distribution may make at most 2^24 RNG calls (rn_generate.cuh: RN_GEN_BUDGET), and a
+ * plan at most 2^26 ops per draw (checked at create).  A chain whose draw would exceed the budget stops: that iteration and
+ * all its later ones in the call are NaN, its state is where the failed draw stopped, and the call returns RN_E_INVALID
+ * naming the first such chain and its iteration (outputs and states are still written; the other chains' draws are
+ * unaffected).  RN_E_LOOKUP as rn_function_eval. */
+typedef struct rn_generator rn_generator;
+int rn_generator_create(const void* rir, size_t len, int device, rn_generator** out);
+int rn_generator_ninputs(const rn_generator* g);
+int rn_generator_noutputs(const rn_generator* g);
+int rn_generator_nslots(const rn_generator* g);
+/* host buffers, blocking: x [chains][iterations][n] -> out [chains][iterations][m_out]; rng_states [chains] in/out */
+int rn_generator_eval(rn_generator* g, const double* x, int64_t iterations, int64_t chains, rn_rng_state* rng_states, double* out);
+/* device-resident draws on `stream` (NULL: the generator's own stream), blocking; rng_states: host [chains] in/out
+ *   RN_LAYOUT_SAMPLER: d_x [iterations][n][chains] as rn_sampler_run wrote it
+ *   RN_LAYOUT_ROWS   : d_x [chains][iterations][n]
+ * d_out: [chains][iterations][m_out] (Trace.predict's order) */
+int rn_generator_eval_device(rn_generator* g, const double* d_x, int layout, int64_t iterations, int64_t chains,
+                             rn_rng_state* rng_states, double* d_out, void* stream);
+/* tooling / tests (no device): the error report of a call from rn_k_generate's per-chain error bits (bit 0: a draw exceeded
+ * the budget) and first failing iterations -- RN_OK, or RN_E_INVALID naming the first failing chain and its iteration */
+int rn_generator_report(const int32_t* err, const int64_t* err_iter, int64_t chains);
+/* iterations per chunk of the slot scratch (0, the default: as many as fit in 256 MB); results do not depend on it */
+int rn_generator_set_chunk(rn_generator* g, int64_t iterations);
+int rn_generator_emit_source(rn_generator* g, char* buf, size_t cap, size_t* needed);
+int rn_generator_emit_cubin(rn_generator* g, void* buf, size_t cap, size_t* needed);
+void rn_generator_destroy(rn_generator* g);
+/* rn_sample_generate   <- model.sample(config).predict(gen) (core/Model.scala:56-63) with the draws of `gen` on the device:
+ * sampling, the slots and the predictive draws in one call; the posterior draws never leave the device.  Chain c's
+ * generator stream starts where its sampling stream ended (the rng of rn_sampler_stats); stats[c].rng is the state after
+ * the predictive draws.  out: host [chains][iterations][m_out].  mass, stats, cfg->diagnostics, cfg->stats_rings as in
+ * rn_sample. */
+int rn_sample_generate(rn_model* m, const rn_config* cfg, rn_generator* g, const int64_t* seeds, int chains, double* out,
+                       double* mass, rn_chain_stats* stats);
+
 /* ---- MAP optimisation: batched multi-start L-BFGS (SURVEY.md 8f-4) ------------------------------------------ */
 /* rn_optimize          <- Optimizer.lbfgs(df: DensityFunction): Array[Double]
  *                         rainier-sampler/.../optimizer/Optimizer.scala:6-24 driving class LBFGS

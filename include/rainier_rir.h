@@ -51,6 +51,11 @@ extern "C" {
  * n_cols == 0 and n_outputs == m >= 1 arbitrary output nodes ("req0".."req{m-1}").  No gradient, no accumulation:
  * output j of a point is the value of node outputs[j].  Consumed by rn_function_create (rainier_cuda.h). */
 #define RIR_FLAG_FUNCTION 2u
+/* RIR_FLAG_GENERATOR (only together with RIR_FLAG_FUNCTION): the container also carries a posterior-predictive generator
+ * plan -- the `Generator.get(rng, evaluator)` half of Trace.predict (core/Trace.scala:34-41) for the built-in
+ * distributions.  The function's m outputs are the plan's "slots": every Real a draw reads.  Consumed by
+ * rn_generator_create (rainier_cuda.h).  The plan section follows the target block (see the file layout below). */
+#define RIR_FLAG_GENERATOR 4u
 
 /* node kinds */
 enum {
@@ -112,11 +117,56 @@ typedef struct rir_target {
 } rir_target; /* 24 bytes + outputs */
 
 /*
+ * Generator plan (RIR_FLAG_GENERATOR).  One draw runs the ops in order over one register `v` (a double) and writes m_out
+ * doubles, in the order of the EMIT ops.  Discrete draws leave a Java Long in v (stored as a double); every double -> long
+ * conversion is the JVM's D2L (NaN -> 0, saturating), double -> int is D2I.  Slot fields name function outputs
+ * ([0, n_outputs)); fields a kind does not read must be -1.  The arithmetic of every op restates the reference
+ * (core/Continuous.scala, core/Discrete.scala) in its own evaluation order.
+ */
+enum {
+  RIR_G_NORMAL = 0,       /* v = RNG.standardNormal                                                  Continuous.scala:63-67   */
+  RIR_G_CAUCHY = 1,       /* v = standardNormal / standardNormal (numerator drawn first)             :72-77           */
+  RIR_G_LAPLACE = 2,      /* u = standardUniform - 0.5; v = signum(u) * -1 * log(1 - 2|u|)           :82-89           */
+  RIR_G_UNIFORM = 3,      /* v = standardUniform                                                     :204-218         */
+  RIR_G_GAMMA = 4,        /* v = Gamma.standard(slot[0]) draw (Marsaglia-Tsang; a < 1 draws u first) :114-144         */
+  RIR_G_BETA = 5,         /* x = Gamma(slot[0], 1), y = Gamma(slot[1], 1) draws; v = x / (x + y)     :162-184         */
+  RIR_G_SCALE = 6,        /* v = v * slot[0]                              (Injection.scala:48-66 fastForwards) */
+  RIR_G_TRANSLATE = 7,    /* v = v + slot[0]                              (Injection.scala:71-86)              */
+  RIR_G_EXP = 8,          /* v = exp(v)                                   (Injection.scala:91-107)             */
+  RIR_G_EMIT = 9,         /* out[next] = v                                                                     */
+  RIR_G_BERNOULLI = 10,   /* slot[0] = p                                                             Discrete.scala:38-52   */
+  RIR_G_GEOMETRIC = 11,   /* slot[0] = p                                                             :59-73           */
+  RIR_G_POISSON = 12,     /* slot[0] = lambda (small below 30, large otherwise)                      :122-186         */
+  RIR_G_BINOMIAL = 13,    /* slots p, k, p*k, k*p, (k*p*(1-p)).pow(0.5), p + 0 (the categorical CDF)  :194-228        */
+  RIR_G_NEGBINOMIAL = 14, /* slots p, n, 1-p, n*p/(1-p), (n*p).pow(1/2)/(1-p)                         :81-108          */
+  RIR_G_VALUE = 15,       /* v = slot[0]                                  (Generator.real, a Real as ToGenerator) */
+  RIR_G_REPEAT = 16,      /* run the ops up to the matching END k times   (Generator.repeat with a constant k)  */
+  RIR_G_END = 17
+};
+#define RIR_G_MAX_SLOTS 6
+#define RIR_G_MAX_DEPTH 8 /* REPEAT nesting */
+
+typedef struct rir_gen_header {
+  uint32_t n_ops;
+  uint32_t m_out;    /* doubles per draw: the EMITs, each multiplied by the k of every enclosing REPEAT; at most 2^24.
+                        Ops executed per draw (likewise multiplied, one more per repetition) are at most 2^26 */
+  uint32_t reserved[2];
+} rir_gen_header; /* 16 bytes */
+
+typedef struct rir_gen_op {
+  uint32_t kind;                  /* RIR_G_* */
+  int32_t slot[RIR_G_MAX_SLOTS];  /* function output indices, -1 where unused */
+  uint32_t reserved;
+  int64_t k;                      /* RIR_G_REPEAT: repetitions, 0 <= k <= INT32_MAX; 0 otherwise */
+} rir_gen_op; /* 40 bytes */
+
+/*
  * File layout:
  *   rir_header
  *   rir_node      nodes[n_nodes]
  *   int32_t       lookup_refs[n_lookup_refs]   (padded to a multiple of 8 bytes)
  *   n_targets x { rir_target, uint32_t outputs[n_outputs] (padded to 8) }
+ *   RIR_FLAG_GENERATOR only: rir_gen_header, rir_gen_op ops[n_ops]
  */
 
 #ifdef __cplusplus

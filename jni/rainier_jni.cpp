@@ -27,6 +27,7 @@
 #include <jni.h>
 
 #include <cstdint>
+#include <cstring>
 #include <memory>
 #include <vector>
 
@@ -182,6 +183,74 @@ JNIEXPORT void JNICALL Java_com_stripe_rainier_cuda_Native_functionEval(JNIEnv* 
 }
 JNIEXPORT void JNICALL Java_com_stripe_rainier_cuda_Native_functionDestroy(JNIEnv*, jclass, jlong h) {
   rn_function_destroy((rn_function*)(intptr_t)h);
+}
+// ---- posterior-predictive draws: Trace.predict's Generator.get on the device (core/Trace.scala:34-41) ----
+// rng states cross as long[3 * chains] = (seed48, doubleToRawLongBits(nextNextGaussian), haveNextNextGaussian) per chain
+static void rng_in(JNIEnv* env, jlongArray a, std::vector<rn_rng_state>& st) {
+  const jsize k = env->GetArrayLength(a) / 3;
+  std::vector<jlong> v((size_t)k * 3);
+  env->GetLongArrayRegion(a, 0, k * 3, v.data());
+  st.assign((size_t)k, rn_rng_state{});
+  for (jsize c = 0; c < k; c++) {
+    st[c].seed48 = v[3 * c];
+    std::memcpy(&st[c].next_gaussian, &v[3 * c + 1], 8);
+    st[c].have_next = (int32_t)v[3 * c + 2];
+  }
+}
+static void rng_out(JNIEnv* env, jlongArray a, const std::vector<rn_rng_state>& st) {
+  std::vector<jlong> v(st.size() * 3);
+  for (size_t c = 0; c < st.size(); c++) {
+    v[3 * c] = st[c].seed48;
+    std::memcpy(&v[3 * c + 1], &st[c].next_gaussian, 8);
+    v[3 * c + 2] = st[c].have_next;
+  }
+  env->SetLongArrayRegion(a, 0, (jsize)v.size(), v.data());
+}
+// def generatorCreate(rir: ByteBuffer, device: Int): Long    (a RIR_FLAG_GENERATOR container)
+JNIEXPORT jlong JNICALL Java_com_stripe_rainier_cuda_Native_generatorCreate(JNIEnv* env, jclass, jobject rir, jint device) {
+  rn_generator* g = nullptr;
+  if (rn_generator_create(env->GetDirectBufferAddress(rir), (size_t)env->GetDirectBufferCapacity(rir), device, &g) != RN_OK) {
+    throw_last(env);
+    return 0;
+  }
+  return (jlong)(intptr_t)g;
+}
+JNIEXPORT jint JNICALL Java_com_stripe_rainier_cuda_Native_generatorOutputs(JNIEnv*, jclass, jlong h) {
+  return rn_generator_noutputs((rn_generator*)(intptr_t)h);
+}
+// def generatorEval(handle: Long, draws: Array[Double] /* [chains][iterations][n] */, iterations: Long, chains: Long,
+//                   rng: Array[Long] /* in/out */, out: Array[Double] /* [chains][iterations][m_out] */): Unit
+JNIEXPORT void JNICALL Java_com_stripe_rainier_cuda_Native_generatorEval(JNIEnv* env, jclass, jlong h, jdoubleArray draws, jlong iterations,
+                                                                         jlong chains, jlongArray rng, jdoubleArray out) {
+  const std::vector<double> vx = in_doubles(env, draws);
+  std::vector<double> vo((size_t)env->GetArrayLength(out));
+  std::vector<rn_rng_state> st;
+  rng_in(env, rng, st);
+  const int rc = rn_generator_eval((rn_generator*)(intptr_t)h, vx.data(), (int64_t)iterations, (int64_t)chains, st.data(), vo.data());
+  if (rc != RN_OK) return throw_last(env);
+  rng_out(env, rng, st);
+  out_doubles(env, out, vo.data(), vo.size());
+}
+JNIEXPORT void JNICALL Java_com_stripe_rainier_cuda_Native_generatorDestroy(JNIEnv*, jclass, jlong h) {
+  rn_generator_destroy((rn_generator*)(intptr_t)h);
+}
+// def sampleGenerate(model: Long, config: ByteBuffer, generator: Long, seeds: Array[Long], out: Array[Double], rngOut: Array[Long]): Unit
+//   model.sample(config).predict(gen) with the draws on the device; rngOut: the states after the predictive draws
+JNIEXPORT void JNICALL Java_com_stripe_rainier_cuda_Native_sampleGenerate(JNIEnv* env, jclass, jlong m, jobject config, jlong g,
+                                                                          jlongArray seeds, jdoubleArray out, jlongArray rngOut) {
+  const jsize chains = env->GetArrayLength(seeds);
+  std::vector<jlong> vs((size_t)chains);
+  env->GetLongArrayRegion(seeds, 0, chains, vs.data());
+  std::vector<int64_t> s64(vs.begin(), vs.end());
+  std::vector<double> vo((size_t)env->GetArrayLength(out));
+  std::vector<rn_chain_stats> stats((size_t)chains);
+  const int rc = rn_sample_generate((rn_model*)(intptr_t)m, (const rn_config*)env->GetDirectBufferAddress(config), (rn_generator*)(intptr_t)g,
+                                    s64.data(), (int)chains, vo.data(), nullptr, stats.data());
+  if (rc != RN_OK) return throw_last(env);
+  std::vector<rn_rng_state> st((size_t)chains);
+  for (jsize c = 0; c < chains; c++) st[c] = stats[c].rng;
+  rng_out(env, rngOut, st);
+  out_doubles(env, out, vo.data(), vo.size());
 }
 // ---- Optimizer.lbfgs for a batch of starts (optimizer/Optimizer.scala:6-24) ----
 // def optimize(handle: Long, x0: Array[Double] /* [starts][n] or null */, starts: Int, m: Int, eps: Double, maxEvals: Int,

@@ -111,6 +111,20 @@ def lib():
         L.rn_function_destroy.argtypes = [C.c_void_p]
         L.rn_sample_predict.argtypes = [C.c_void_p, C.POINTER(Config), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                         C.c_void_p]
+        L.rn_generator_create.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(C.c_void_p)]
+        L.rn_generator_ninputs.argtypes = [C.c_void_p]
+        L.rn_generator_noutputs.argtypes = [C.c_void_p]
+        L.rn_generator_nslots.argtypes = [C.c_void_p]
+        L.rn_generator_eval.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]
+        L.rn_generator_eval_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
+                                               C.c_void_p]
+        L.rn_generator_set_chunk.argtypes = [C.c_void_p, C.c_int64]
+        L.rn_generator_report.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
+        L.rn_generator_emit_source.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.rn_generator_emit_cubin.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.rn_generator_destroy.argtypes = [C.c_void_p]
+        L.rn_sample_generate.argtypes = [C.c_void_p, C.POINTER(Config), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                         C.c_void_p]
         sizes = (C.c_int32 * 4)()
         L.rn_abi_sizes(sizes)
         if sizes[0] != C.sizeof(Config) or sizes[1] != C.sizeof(ChainStats) or sizes[2] != C.sizeof(RngState):
@@ -368,6 +382,12 @@ class Trace:
         c = np.ascontiguousarray(self.chains, dtype=np.float64)
         return function(c.reshape(-1, c.shape[-1]))
 
+    def generate(self, generator, rng_states):
+        """Trace.predict (core/Trace.scala:34-41) with the draws on the device: chain c continues rng_states[c] (one
+        RngState, or a (seed48, next_gaussian, have_next) tuple, per chain).  Returns (draws [chains][iterations][m_out],
+        the RngStates after the last draw)."""
+        return generator(self.chains, rng_states)
+
 
 # ----------------------------------------------------------------------------------------------------------
 # compiled functions (posterior-predictive requirements)
@@ -439,6 +459,85 @@ class CudaFunction:
         out = (C.c_double * 2)()
         _check(lib().rn_function_op_counts(self.h, out))
         return {"flops": out[0], "special": out[1]}
+
+
+def _rng_array(rng_states):
+    states = [st if isinstance(st, RngState) else RngState(int(st[0]), float(st[1]), int(st[2]), 0) for st in rng_states]
+    return (RngState * max(len(states), 1))(*states), len(states)
+
+
+def generator_report(err, err_iter):
+    """tooling / tests (no device): rn_generator_report -- raises RainierCudaError(RN_E_INVALID) naming the first chain whose
+    error bit 0 (a draw over the RNG budget) is set, as rn_generator_eval does after its launches"""
+    err = np.ascontiguousarray(err, dtype=np.int32)
+    err_iter = np.ascontiguousarray(err_iter, dtype=np.int64)
+    _check(lib().rn_generator_report(err.ctypes.data, err_iter.ctypes.data, len(err)))
+
+
+class CudaGenerator:
+    """The Generator.get half of Trace.predict on the device (rn_generator_*): a RIR_FLAG_GENERATOR container (built by
+    rainier_b200.generate.lower_generator) -> the slots' rn_function() + rn_k_eval and the plan's rn_k_generate, one thread
+    per chain continuing that chain's java.util.Random stream."""
+
+    def __init__(self, rir, device=0):
+        L = lib()
+        self._rir = bytes(rir)
+        h = C.c_void_p()
+        _check(L.rn_generator_create(self._rir, len(self._rir), int(device), C.byref(h)))
+        self.h = h
+        self.nInputs = L.rn_generator_ninputs(h)
+        self.nOutputs = L.rn_generator_noutputs(h)
+        self.nSlots = L.rn_generator_nslots(h)
+        self.device = device
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().rn_generator_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __call__(self, x, rng_states):
+        """x: [chains][iterations][nInputs] host array; rng_states: one per chain.  Returns (out [chains][iterations][nOutputs],
+        list of RngState after the draws)."""
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        chains, iterations = x.shape[0], x.shape[1]
+        arr, k = _rng_array(rng_states)
+        if k != chains:
+            raise ValueError("one rng state per chain")
+        out = np.empty((chains, iterations, self.nOutputs), dtype=np.float64)
+        _check(lib().rn_generator_eval(self.h, x.ctypes.data, iterations, chains, C.cast(arr, C.c_void_p), out.ctypes.data))
+        return out, list(arr)[:chains]
+
+    def eval_device(self, d_x, iterations, chains, rng_states, d_out, layout=abi.RN_LAYOUT_SAMPLER, stream=None):
+        """device pointers (ints); blocking.  Returns the RngStates after the draws."""
+        arr, k = _rng_array(rng_states)
+        if k != chains:
+            raise ValueError("one rng state per chain")
+        _check(lib().rn_generator_eval_device(self.h, C.c_void_p(d_x), layout, iterations, chains, C.cast(arr, C.c_void_p),
+                                              C.c_void_p(d_out), C.c_void_p(stream) if stream else None))
+        return list(arr)[:chains]
+
+    def set_chunk(self, iterations):
+        _check(lib().rn_generator_set_chunk(self.h, int(iterations)))
+
+    def emit_source(self):
+        need = C.c_size_t()
+        _check(lib().rn_generator_emit_source(self.h, None, 0, C.byref(need)))
+        buf = C.create_string_buffer(need.value)
+        _check(lib().rn_generator_emit_source(self.h, buf, need.value, C.byref(need)))
+        return buf.value.decode()
+
+    def emit_cubin(self):
+        need = C.c_size_t()
+        _check(lib().rn_generator_emit_cubin(self.h, None, 0, C.byref(need)))
+        buf = C.create_string_buffer(need.value)
+        _check(lib().rn_generator_emit_cubin(self.h, buf, need.value, C.byref(need)))
+        return buf.raw
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -569,6 +668,27 @@ class CudaModel:
         _check(lib().rn_sample_predict(self.h, C.byref(cfg), function.h, seeds_a.ctypes.data, nChains, pred.ctypes.data,
                                        mass.ctypes.data, C.cast(stats, C.c_void_p)))
         return pred, Trace(None, mass, [Stats(stats[c], rings[c]) for c in range(nChains)])
+
+    def sample_generate(self, generator, config=None, nChains=4, seeds=None, out=None):
+        """model.sample(config).predict(gen) with the predictive draws on the device (rn_sample_generate): returns
+        (draws [chains][iterations][m_out], Trace without chains).  Chain c's draws continue its sampling RNG stream;
+        Trace.stats[c].rng is the state after them.  Only the predictive draws cross PCIe."""
+        config = config or SamplerConfig()
+        cfg, keep = lower_config(config)
+        if seeds is None:
+            seeds = np.arange(nChains, dtype=np.int64) + 1
+        seeds_a = np.ascontiguousarray(seeds, dtype=np.int64)
+        nChains = len(seeds_a)
+        n = self.nVars
+        dense = cfg.mass_tuner == abi.RN_MASS_DENSE or (cfg.mass_tuner == abi.RN_MASS_STATIC and cfg.static_matrix == abi.RN_MATRIX_DENSE)
+        draws = out if out is not None else np.empty((nChains, cfg.iterations, generator.nOutputs), dtype=np.float64)
+        mass = np.empty((nChains, n * n if dense else n), dtype=np.float64)
+        stats = (ChainStats * nChains)()
+        rings = np.zeros((nChains, 3, cfg.stats_window), dtype=np.float64)
+        cfg.stats_rings = rings.ctypes.data_as(C.POINTER(C.c_double))
+        _check(lib().rn_sample_generate(self.h, C.byref(cfg), generator.h, seeds_a.ctypes.data, nChains, draws.ctypes.data,
+                                        mass.ctypes.data, C.cast(stats, C.c_void_p)))
+        return draws, Trace(None, mass, [Stats(stats[c], rings[c]) for c in range(nChains)])
 
     # -- Model.optimize / Optimizer.lbfgs, batched over starts --
     @staticmethod

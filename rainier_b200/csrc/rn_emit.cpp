@@ -19,6 +19,7 @@ extern const char* kSamplerSource;        // rn_sampler.cuh + rn_diag.cuh
 extern const char* kSamplerWpcSource;     // rn_sampler_wpc.cuh + rn_diag.cuh
 extern const char* kFunctionSource;    // rn_function.cuh
 extern const char* kOptimizerSource;   // rn_args.h + rn_optimizer.cuh
+extern const char* kGenerateSource;    // rn_gen_args.h + rn_generate.cuh
 
 namespace {
 
@@ -1875,6 +1876,68 @@ std::string emit_function_source(const Program& P, const EmitOptions& opt) {
   Emitter E(P, opt);
   E.function_tpc();
   os << E.os.str() << "\n" << kFunctionSource << "\n";
+  return os.str();
+}
+
+std::string emit_generator_source(const Program& P, const GeneratorPlan& G) {
+  std::ostringstream os;
+  os << "// generated by rainier_b200 (CUDA source emitter, generator flavour) -- do not edit\n";
+  os << "#define RN_N " << P.n_params << "\n";
+  os << "#define RN_NQ " << std::max<uint32_t>(1, P.n_params) << "\n";
+  os << "#define RN_M " << P.fn_outputs.size() << "\n";
+  os << "#define RN_MOUT " << G.m_out << "\n";
+  os << "#define RN_BACKEND 0\n";
+  os << kPreludeSource << "\n";
+  EmitOptions eo;
+  Emitter E(P, eo);
+  E.function_tpc();
+  os << E.os.str() << "\n" << kFunctionSource << "\n" << kGenerateSource << "\n";
+  os << "// ---- emitted: the generator plan (" << G.ops.size() << " ops, " << G.m_out << " values per draw) ----\n";
+  os << "RN_DEVICE void rn_generate(RnGen& g, const double* RN_RESTRICT s, const long long ss, double* RN_RESTRICT o) {\n";
+  os << "  double v = 0.0;\n  long long j = 0;\n";
+  auto sl = [](int32_t k) { return "s[" + std::to_string(k) + "LL * ss]"; };
+  int depth = 0;
+  for (const rir_gen_op& o : G.ops) {
+    const std::string ind(2 * (depth + 1), ' ');
+    const int32_t* q = o.slot;
+    switch (o.kind) {
+      case RIR_G_NORMAL: os << ind << "g.calls = 0;\n" << ind << "v = rn_g_normal_draw(g);\n"; break;
+      case RIR_G_CAUCHY: os << ind << "g.calls = 0;\n" << ind << "v = rn_g_cauchy(g);\n"; break;
+      case RIR_G_LAPLACE: os << ind << "g.calls = 0;\n" << ind << "v = rn_g_laplace(g);\n"; break;
+      case RIR_G_UNIFORM: os << ind << "g.calls = 0;\n" << ind << "v = rn_g_uniform_draw(g);\n"; break;
+      case RIR_G_GAMMA: os << ind << "v = rn_g_gamma(g, " << sl(q[0]) << ");\n"; break;
+      case RIR_G_BETA: os << ind << "v = rn_g_beta(g, " << sl(q[0]) << ", " << sl(q[1]) << ");\n"; break;
+      case RIR_G_SCALE: os << ind << "v = v * " << sl(q[0]) << ";\n"; break;
+      case RIR_G_TRANSLATE: os << ind << "v = v + " << sl(q[0]) << ";\n"; break;
+      case RIR_G_EXP: os << ind << "v = rn_exp(v);\n"; break;
+      case RIR_G_EMIT: os << ind << "o[j++] = v;\n"; break;
+      case RIR_G_BERNOULLI: os << ind << "v = rn_g_bernoulli_op(g, " << sl(q[0]) << ");\n"; break;
+      case RIR_G_GEOMETRIC: os << ind << "v = rn_g_geometric(g, " << sl(q[0]) << ");\n"; break;
+      case RIR_G_POISSON: os << ind << "v = rn_g_poisson(g, " << sl(q[0]) << ");\n"; break;
+      case RIR_G_BINOMIAL:
+        os << ind << "v = rn_g_binomial(g";
+        for (int k = 0; k < 6; k++) os << ", " << sl(q[k]);
+        os << ");\n";
+        break;
+      case RIR_G_NEGBINOMIAL:
+        os << ind << "v = rn_g_negbinomial(g";
+        for (int k = 0; k < 5; k++) os << ", " << sl(q[k]);
+        os << ");\n";
+        break;
+      case RIR_G_VALUE: os << ind << "v = " << sl(q[0]) << ";\n"; break;
+      case RIR_G_REPEAT:
+        os << ind << "for (long long r" << depth << " = 0; r" << depth << " < " << o.k << "LL; r" << depth << "++) {\n";
+        depth++;
+        break;
+      case RIR_G_END:
+        depth--;
+        os << std::string(2 * (depth + 1), ' ') << "}\n";
+        break;
+    }
+    const bool draws = (o.kind <= RIR_G_BETA) || (o.kind >= RIR_G_BERNOULLI && o.kind <= RIR_G_NEGBINOMIAL);
+    if (draws) os << ind << "if (g.bad) return;\n";
+  }
+  os << "  (void)v;\n  (void)j;\n}\n";
   return os.str();
 }
 

@@ -39,6 +39,9 @@ std::string emit_source(const Program& P, const EmitOptions& opt);
 // function flavour (Program from build_function): prelude + emitted rn_function() + rn_function.cuh (rn_k_eval); only
 // opt.fast_math is read
 std::string emit_function_source(const Program& P, const EmitOptions& opt);
+// generator flavour (build_generator): the function flavour's rn_function() + rn_k_eval (the slots), rn_generate.cuh and the
+// plan emitted as straight-line rn_generate() (REPEAT as a counted loop).  Parity math only.
+std::string emit_generator_source(const Program& P, const GeneratorPlan& G);
 // optimizer flavour: prelude + emitted thread-per-chain rn_density() + rn_optimizer.cuh (rn_k_lbfgs, `history` = the m of
 // new LBFGS(x, m, eps)); reads opt.fast_math and opt.target_base
 std::string emit_optimizer_source(const Program& P, const EmitOptions& opt, int history);

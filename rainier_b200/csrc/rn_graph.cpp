@@ -657,6 +657,86 @@ std::string build_function(const void* rir, size_t len, Program& P) {
   return "";
 }
 
+std::string build_generator(const void* rir, size_t len, Program& P, GeneratorPlan& G) {
+  if (!rir || len < sizeof(rir_header)) return "RIR: truncated header";
+  rir_header h;
+  std::memcpy(&h, rir, sizeof(h));
+  if (!(h.flags & RIR_FLAG_GENERATOR)) return "RIR: not a generator container (RIR_FLAG_GENERATOR clear)";
+  std::string e = build_function(rir, len, P);
+  if (!e.empty()) return e;
+  // the plan section starts after the (single) target block, whose sizes build_function has checked
+  size_t off = sizeof(h) + (size_t)h.n_nodes * sizeof(rir_node) + (((size_t)h.n_lookup_refs * 4 + 7) & ~(size_t)7);
+  rir_target rt;
+  std::memcpy(&rt, (const uint8_t*)rir + off, sizeof(rt));
+  off += sizeof(rt) + (((size_t)rt.n_outputs * 4 + 7) & ~(size_t)7);
+  rir_gen_header gh;
+  if (len - off < sizeof(gh)) return "RIR: truncated generator header";
+  std::memcpy(&gh, (const uint8_t*)rir + off, sizeof(gh));
+  off += sizeof(gh);
+  if (gh.n_ops == 0) return "RIR: generator without ops";
+  if ((len - off) / sizeof(rir_gen_op) < gh.n_ops) return "RIR: truncated generator ops";
+  G = GeneratorPlan();
+  G.ops.resize(gh.n_ops);
+  std::memcpy(G.ops.data(), (const uint8_t*)rir + off, (size_t)gh.n_ops * sizeof(rir_gen_op));
+  const int64_t m = (int64_t)P.fn_outputs.size();
+  // slots each kind reads; the remaining fields must be -1
+  auto arity = [](uint32_t kind) -> int {
+    switch (kind) {
+      case RIR_G_GAMMA: case RIR_G_SCALE: case RIR_G_TRANSLATE: case RIR_G_BERNOULLI: case RIR_G_GEOMETRIC:
+      case RIR_G_POISSON: case RIR_G_VALUE: return 1;
+      case RIR_G_BETA: return 2;
+      case RIR_G_NEGBINOMIAL: return 5;
+      case RIR_G_BINOMIAL: return 6;
+      default: return 0;
+    }
+  };
+  // per draw: at most 2^24 values and 2^26 ops executed (an op inside REPEATs counts once per repetition, a repetition
+  // itself once), so that no container makes one draw run unboundedly long whatever its RNG budget
+  const int64_t kMaxOut = (int64_t)1 << 24;
+  const double kMaxExecuted = (double)((int64_t)1 << 26);
+  int64_t mult[RIR_G_MAX_DEPTH + 1], emitted[RIR_G_MAX_DEPTH + 1];
+  double executed[RIR_G_MAX_DEPTH + 1];
+  int depth = 0;
+  mult[0] = 1;
+  emitted[0] = 0;
+  executed[0] = 0;
+  for (size_t i = 0; i < G.ops.size(); i++) {
+    const rir_gen_op& o = G.ops[i];
+    if (o.kind > RIR_G_END) return "RIR: unknown generator op kind at op " + std::to_string(i);
+    const int a = arity(o.kind);
+    for (int s = 0; s < RIR_G_MAX_SLOTS; s++) {
+      if (s < a && (o.slot[s] < 0 || o.slot[s] >= m)) return "RIR: generator slot out of range at op " + std::to_string(i);
+      if (s >= a && o.slot[s] != -1) return "RIR: unused generator slot field is not -1 at op " + std::to_string(i);
+    }
+    if (o.kind != RIR_G_REPEAT && o.k != 0) return "RIR: repeat count on a non-REPEAT op at op " + std::to_string(i);
+    if (o.kind == RIR_G_REPEAT) {
+      if (o.k < 0 || o.k > 2147483647LL) return "RIR: REPEAT count out of range at op " + std::to_string(i);
+      if (depth == RIR_G_MAX_DEPTH) return "RIR: REPEAT nested too deeply at op " + std::to_string(i);
+      depth++;
+      mult[depth] = o.k;
+      emitted[depth] = 0;
+      executed[depth] = 1;
+    } else if (o.kind == RIR_G_END) {
+      if (depth == 0) return "RIR: END without REPEAT at op " + std::to_string(i);
+      const int64_t inner = emitted[depth] * mult[depth];
+      const double inner_ops = executed[depth] * (double)mult[depth];
+      depth--;
+      emitted[depth] += inner;
+      executed[depth] += inner_ops;
+    } else {
+      if (o.kind == RIR_G_EMIT) emitted[depth] += 1;
+      executed[depth] += 1;
+    }
+    if (emitted[depth] > kMaxOut) return "RIR: generator emits more than 2^24 values per draw";
+    if (executed[depth] > kMaxExecuted) return "RIR: generator executes more than 2^26 ops per draw";
+  }
+  if (depth != 0) return "RIR: REPEAT without END";
+  if (emitted[0] == 0) return "RIR: generator emits nothing";
+  if ((int64_t)gh.m_out != emitted[0]) return "RIR: generator m_out does not match its EMIT ops";
+  G.m_out = gh.m_out;
+  return "";
+}
+
 SeparableInfo analyze_separable(const Program& P, int max_degree, int max_atoms) {
   SeparableInfo R;
   const int N = (int)P.nodes.size();

@@ -134,4 +134,12 @@ SeparableInfo analyze_separable(const Program& P, int max_degree = 2, int max_at
 // fn_outputs / counts.flops_inv, special_inv.
 std::string build_function(const void* rir, size_t len, Program& out);
 
+// RIR_FLAG_GENERATOR containers: the function of build_function (its outputs are the plan's slots) followed by the
+// generator plan of rainier_rir.h.  Every op kind, slot index, REPEAT count and nesting, and m_out are validated here.
+struct GeneratorPlan {
+  std::vector<rir_gen_op> ops;
+  uint32_t m_out = 0;
+};
+std::string build_generator(const void* rir, size_t len, Program& fn, GeneratorPlan& plan);
+
 }  // namespace rn

@@ -3137,3 +3137,329 @@ extern "C" int rn_sample_predict(rn_model* m, const rn_config* cfg, rn_function*
   }
   return rn_sampler_stats(s, stats, mass, cfg->stats_rings);
 }
+
+// ---------------------------------------------------------------------------------------------------------
+// rn_generator: the other half of Trace.predict (rainier-core/.../core/Trace.scala:34-41) -- `Generator.get(rng, evaluator)`
+// for every posterior draw, on the device, for the built-in distributions (rn_generate.cuh).  One module holds the slots'
+// function (rn_k_eval) and the draws (rn_k_generate).  A call walks its iterations in chunks: rn_k_eval writes the slot values
+// of a chunk [iteration][slot][chain] into a scratch of at most kGenScratchBytes, rn_k_generate continues every chain's RNG
+// over the chunk.  By the stream rule the chunking is invisible in the results.
+// ---------------------------------------------------------------------------------------------------------
+#include "rn_gen_args.h"
+
+static const size_t kGenScratchBytes = (size_t)256 << 20;
+static const int kGenBudget = 1 << 24;  // RN_GEN_BUDGET of rn_generate.cuh
+static_assert(sizeof(RnRngState) == sizeof(rn_rng_state), "RnRngState mirrors rn_rng_state");
+
+struct rn_generator {
+  Program prog;
+  GeneratorPlan plan;
+  int device = -1;
+  CUcontext ctx = nullptr;
+  std::string source;
+  std::vector<char> cubin;
+  CUmodule mod = nullptr;
+  CUfunction k_eval = nullptr, k_gen = nullptr;
+  CUstream stream = nullptr;
+  int sm_count = 132;
+  int64_t chunk = 0;  // iterations per chunk; 0 = from kGenScratchBytes
+  // grow-only device buffers: the slot scratch, and per chain the RNG state, error bits and first failing iteration (plus the
+  // lookup flag of rn_k_eval), laid out [rng C][err C, padded to 8 bytes][err_iter C][lookup]
+  CUdeviceptr slots = 0, state = 0;
+  size_t slots_bytes = 0;
+  int64_t state_chains = 0;
+};
+
+static int generator_load(const Api* A, rn_generator* g) {
+  CU(A->cuCtxSetCurrent(g->ctx));
+  if (g->mod) return RN_OK;
+  if (g->cubin.empty()) {
+    int rc = nvrtc_to_cubin(g->source, "rainier_generator.cu", false, g->cubin);
+    if (rc) return rc;
+  }
+  CU(A->cuModuleLoadData(&g->mod, g->cubin.data()));
+  CU(A->cuModuleGetFunction(&g->k_eval, g->mod, "rn_k_eval"));
+  CU(A->cuModuleGetFunction(&g->k_gen, g->mod, "rn_k_generate"));
+  CU(A->cuStreamCreate(&g->stream, 1 /*CU_STREAM_NON_BLOCKING*/));
+  CUdevice dev;
+  int sms = 0;
+  if (A->cuDeviceGet(&dev, g->device) == 0 && A->cuDeviceGetAttribute(&sms, 16 /*MULTIPROCESSOR_COUNT*/, dev) == 0 && sms > 0)
+    g->sm_count = sms;
+  return RN_OK;
+}
+
+// the per-chain error bits of rn_k_generate -> RN_E_INVALID naming the first failing chain and its iteration
+static int generator_report(const int32_t* err, const int64_t* err_iter, int64_t chains) {
+  for (int64_t c = 0; c < chains; c++)
+    if (err[c] & 1)
+      return fail(RN_E_INVALID, "generator draw of chain " + std::to_string(c) + ", iteration " + std::to_string(err_iter[c]) +
+                                    " exceeded its budget of " + std::to_string(kGenBudget) + " RNG calls (parameter values on which the "
+                                    "reference would not terminate); the chain's later draws are NaN");
+  return RN_OK;
+}
+
+// the draws of `iterations` x `chains` posterior draws d_x (layout as rn_generator_eval_device) into d_out, continuing
+// rng_states (host, in/out); blocking.  The slot scratch holds at most kGenScratchBytes: blocks of chains when one
+// iteration's slots of all chains exceed it, chunks of iterations within a block.
+static int generator_run(const Api* A, rn_generator* g, const double* d_x, int layout, int64_t iterations, int64_t chains,
+                         rn_rng_state* rng_states, double* d_out, CUstream st) {
+  int rc = generator_load(A, g);
+  if (rc) return rc;
+  const long long n = (long long)g->prog.n_params, M = (long long)g->prog.fn_outputs.size(), C = chains, I = iterations,
+                  mo = (long long)g->plan.m_out;
+  if (C == 0) return RN_OK;
+  const long long budget = (long long)kGenScratchBytes;
+  const long long Cb = std::min<long long>(C, std::max<long long>(1, budget / (M * 8)));  // chains per block
+  long long chunk = g->chunk > 0 ? g->chunk : std::max<long long>(1, budget / (M * Cb * 8));
+  chunk = std::max<long long>(1, std::min<long long>(chunk, std::max<long long>(I, 1)));
+  if (!st) st = g->stream;
+  const size_t need_slots = (size_t)(chunk * M * Cb * 8);
+  if (I > 0 && g->slots_bytes < need_slots) {
+    if (g->slots) A->cuMemFree(g->slots);
+    g->slots = 0;
+    g->slots_bytes = 0;
+    CU(A->cuMemAlloc(&g->slots, need_slots));
+    g->slots_bytes = need_slots;
+  }
+  if (g->state_chains < C) {
+    if (g->state) A->cuMemFree(g->state);
+    g->state = 0;
+    g->state_chains = 0;
+    CU(A->cuMemAlloc(&g->state, (size_t)C * (sizeof(rn_rng_state) + 8) + (((size_t)C * 4 + 7) & ~(size_t)7) + 8));
+    g->state_chains = C;
+  }
+  // the int32 error bits are padded to 8 bytes so that the int64 iterations after them stay 8-byte aligned for any C
+  const CUdeviceptr d_rng = g->state, d_err = d_rng + (size_t)C * sizeof(rn_rng_state),
+                    d_err_iter = d_err + (((size_t)C * 4 + 7) & ~(size_t)7), d_lookup = d_err_iter + (size_t)C * 8;
+  CU(A->cuMemcpyHtoDAsync(d_rng, rng_states, (size_t)C * sizeof(rn_rng_state), st));
+  CU(A->cuMemsetD8Async(d_err, 0, (size_t)C * 4, st));
+  CU(A->cuMemsetD8Async(d_err_iter, 0xff, (size_t)C * 8, st));  // -1
+  CU(A->cuMemsetD8Async(d_lookup, 0, 8, st));
+  for (long long c0 = 0; c0 < C; c0 += Cb) {
+    const long long cb = std::min(Cb, C - c0);
+    for (long long t0 = 0; t0 < I; t0 += chunk) {
+      const long long cnt = std::min(chunk, I - t0);
+      RnEvalArgs e;
+      std::memset(&e, 0, sizeof(e));
+      e.count = cnt * cb;  // point p = (t - t0) * cb + (c - c0)
+      if (layout == RN_LAYOUT_SAMPLER) {  // [iteration][n][chain]
+        e.x = d_x ? d_x + t0 * n * C + c0 : nullptr;
+        e.in_inner = cb, e.in_outer = n * C, e.in_pstride = 1, e.in_estride = C;
+      } else {  // [chain][iteration][n]
+        e.x = d_x ? d_x + c0 * I * n + t0 * n : nullptr;
+        e.in_inner = cb, e.in_outer = n, e.in_pstride = I * n, e.in_estride = 1;
+      }
+      e.out = (double*)(uintptr_t)g->slots;
+      e.out_inner = cb, e.out_outer = M * cb, e.out_pstride = 1, e.out_estride = cb;  // [iteration][slot][chain]
+      e.err = (int*)(uintptr_t)d_lookup;
+      const unsigned grid_e = (unsigned)std::max<long long>(1, std::min<long long>((e.count + 127) / 128, (long long)g->sm_count * 16));
+      void* pe[] = {&e};
+      CU(A->cuLaunchKernel(g->k_eval, grid_e, 1, 1, 128, 1, 1, 0, st, pe, nullptr));
+      RnGenArgs a;
+      a.slots = (const double*)(uintptr_t)g->slots;
+      a.out = d_out + c0 * I * mo;
+      a.rng = (RnRngState*)(uintptr_t)d_rng + c0;
+      a.err = (int*)(uintptr_t)d_err + c0;
+      a.err_iter = (long long*)(uintptr_t)d_err_iter + c0;
+      a.chains = cb, a.t0 = t0, a.t1 = t0 + cnt, a.iterations = I;
+      void* pg[] = {&a};
+      CU(A->cuLaunchKernel(g->k_gen, (unsigned)((cb + 127) / 128), 1, 1, 128, 1, 1, 0, st, pg, nullptr));
+    }
+  }
+  std::vector<int32_t> err((size_t)C);
+  std::vector<int64_t> err_iter((size_t)C);
+  int lookup = 0;
+  CU(A->cuMemcpyDtoHAsync(rng_states, d_rng, (size_t)C * sizeof(rn_rng_state), st));
+  CU(A->cuMemcpyDtoHAsync(err.data(), d_err, (size_t)C * 4, st));
+  CU(A->cuMemcpyDtoHAsync(err_iter.data(), d_err_iter, (size_t)C * 8, st));
+  CU(A->cuMemcpyDtoHAsync(&lookup, d_lookup, 4, st));
+  CU(A->cuStreamSynchronize(st));
+  if (lookup & 1) return fail(RN_E_LOOKUP, "lookup index out of range in a generator slot");
+  return generator_report(err.data(), err_iter.data(), C);
+}
+
+extern "C" {
+
+int rn_generator_create(const void* rir, size_t len, int device, rn_generator** out) {
+  if (!rir || !out) return fail(RN_E_INVALID, "null argument");
+  std::unique_ptr<rn_generator> g(new rn_generator());
+  std::string e = build_generator(rir, len, g->prog, g->plan);
+  if (!e.empty()) return fail(RN_E_INVALID, e);
+  g->source = emit_generator_source(g->prog, g->plan);
+  g->device = device;
+  if (device >= 0) {
+    std::string why;
+    const Api* A = api(&why);
+    if (!A) return fail(RN_E_CUDA, why);
+    int rc = host_ctx(A, device);
+    if (rc) return rc;
+    CUdevice dev;
+    CU(A->cuDeviceGet(&dev, device));
+    CU(A->cuDevicePrimaryCtxRetain(&g->ctx, dev));
+  }
+  *out = g.release();
+  return RN_OK;
+}
+
+int rn_generator_ninputs(const rn_generator* g) { return g ? (int)g->prog.n_params : RN_E_INVALID; }
+int rn_generator_noutputs(const rn_generator* g) { return g ? (int)g->plan.m_out : RN_E_INVALID; }
+int rn_generator_nslots(const rn_generator* g) { return g ? (int)g->prog.fn_outputs.size() : RN_E_INVALID; }
+
+int rn_generator_report(const int32_t* err, const int64_t* err_iter, int64_t chains) {
+  if (chains < 0 || (chains > 0 && (!err || !err_iter))) return fail(RN_E_INVALID, "bad argument");
+  return generator_report(err, err_iter, chains);
+}
+
+int rn_generator_set_chunk(rn_generator* g, int64_t iterations) {
+  if (!g || iterations < 0) return fail(RN_E_INVALID, "bad argument");
+  g->chunk = iterations;
+  return RN_OK;
+}
+
+int rn_generator_emit_source(rn_generator* g, char* buf, size_t cap, size_t* needed) {
+  if (!g) return fail(RN_E_INVALID, "null generator");
+  if (needed) *needed = g->source.size() + 1;
+  if (buf && cap) {
+    size_t k = std::min(cap - 1, g->source.size());
+    std::memcpy(buf, g->source.data(), k);
+    buf[k] = 0;
+  }
+  return RN_OK;
+}
+
+int rn_generator_emit_cubin(rn_generator* g, void* buf, size_t cap, size_t* needed) {
+  if (!g) return fail(RN_E_INVALID, "null generator");
+  if (g->cubin.empty()) {
+    int rc = nvrtc_to_cubin(g->source, "rainier_generator.cu", false, g->cubin);
+    if (rc) return rc;
+  }
+  if (needed) *needed = g->cubin.size();
+  if (buf && cap) std::memcpy(buf, g->cubin.data(), std::min(cap, g->cubin.size()));
+  return RN_OK;
+}
+
+int rn_generator_eval_device(rn_generator* g, const double* d_x, int layout, int64_t iterations, int64_t chains,
+                             rn_rng_state* rng_states, double* d_out, void* stream) {
+  if (!g || iterations < 0 || chains < 0) return fail(RN_E_INVALID, "bad argument");
+  if (layout != RN_LAYOUT_SAMPLER && layout != RN_LAYOUT_ROWS) return fail(RN_E_INVALID, "unknown layout");
+  if (g->device < 0) return fail(RN_E_CUDA, "generator was created without a device (no CPU fallback)");
+  if (chains > 0 && !rng_states) return fail(RN_E_INVALID, "null rng states");
+  if (iterations > 0 && chains > 0 && (!d_out || (!d_x && g->prog.n_params > 0))) return fail(RN_E_INVALID, "null buffer");
+  std::string why;
+  const Api* A = api(&why);
+  if (!A) return fail(RN_E_CUDA, why);
+  return generator_run(A, g, d_x, layout, iterations, chains, rng_states, d_out, (CUstream)stream);
+}
+
+int rn_generator_eval(rn_generator* g, const double* x, int64_t iterations, int64_t chains, rn_rng_state* rng_states, double* out) {
+  if (!g || iterations < 0 || chains < 0) return fail(RN_E_INVALID, "bad argument");
+  if (g->device < 0) return fail(RN_E_CUDA, "generator was created without a device (no CPU fallback)");
+  if (chains > 0 && !rng_states) return fail(RN_E_INVALID, "null rng states");
+  const size_t n = g->prog.n_params, mo = g->plan.m_out, count = (size_t)iterations * (size_t)chains;
+  if (count > 0 && (!out || (!x && n > 0))) return fail(RN_E_INVALID, "null buffer");
+  std::string why;
+  const Api* A = api(&why);
+  if (!A) return fail(RN_E_CUDA, why);
+  int rc = generator_load(A, g);
+  if (rc) return rc;
+  struct Bufs {
+    const Api* A;
+    CUdeviceptr x = 0, out = 0;
+    ~Bufs() {
+      if (x) A->cuMemFree(x);
+      if (out) A->cuMemFree(out);
+    }
+  } b{A};
+  if (count > 0) {
+    if (n > 0) {
+      CU(A->cuMemAlloc(&b.x, count * n * 8));
+      CU(A->cuMemcpyHtoD(b.x, x, count * n * 8));
+    }
+    CU(A->cuMemAlloc(&b.out, count * mo * 8));
+  }
+  rc = generator_run(A, g, (const double*)(uintptr_t)b.x, RN_LAYOUT_ROWS, iterations, chains, rng_states, (double*)(uintptr_t)b.out,
+                     g->stream);
+  if (count > 0) CU(A->cuMemcpyDtoH(out, b.out, count * mo * 8));  // what was drawn, also when a draw exceeded its budget
+  return rc;
+}
+
+void rn_generator_destroy(rn_generator* g) {
+  if (!g) return;
+  std::string why;
+  const Api* A = g->device >= 0 ? api(&why) : nullptr;
+  if (A && g->ctx) {
+    A->cuCtxSetCurrent(g->ctx);
+    if (g->stream) {
+      A->cuStreamSynchronize(g->stream);
+      A->cuStreamDestroy(g->stream);
+    }
+    if (g->mod) A->cuModuleUnload(g->mod);
+    if (g->slots) A->cuMemFree(g->slots);
+    if (g->state) A->cuMemFree(g->state);
+    CUdevice dev;
+    if (A->cuDeviceGet(&dev, g->device) == 0) A->cuDevicePrimaryCtxRelease(dev);
+  }
+  delete g;
+}
+
+// rn_sample_generate: model.sample(config).predict(gen) with the draws of the generator on the device as well.  Built from the
+// staged entry points like rn_sample_predict; every chain's generator stream starts where its sampling stream ended.
+int rn_sample_generate(rn_model* m, const rn_config* cfg, rn_generator* g, const int64_t* seeds, int chains, double* out,
+                       double* mass, rn_chain_stats* stats) {
+  if (!m) return fail(RN_E_INVALID, "null model");
+  std::lock_guard<std::recursive_mutex> model_lock_(m->mu);
+  if (!cfg || !g || chains <= 0 || cfg->iterations < 0) return fail(RN_E_INVALID, "bad argument");
+  if (!out && cfg->iterations > 0) return fail(RN_E_INVALID, "null output buffer");
+  if (m->device < 0 || g->device < 0) return fail(RN_E_CUDA, "model/generator was created without a device (no CPU fallback)");
+  if (m->device != g->device) return fail(RN_E_INVALID, "model and generator live on different devices");
+  if (g->prog.n_params != m->n_params) return fail(RN_E_INVALID, "the generator's inputs are not the model's parameters");
+  std::string why;
+  const Api* A = api(&why);
+  if (!A) return fail(RN_E_CUDA, why);
+  rn_sampler* s = nullptr;
+  int rc = rn_sampler_create(m, cfg, seeds, chains, &s);
+  if (rc) return rc;
+  struct Guard {
+    rn_sampler* s;
+    ~Guard() { rn_sampler_destroy(s); }
+  } guard{s};
+  rc = rn_sampler_warmup(s, -1);
+  if (rc) return rc;
+  rc = rn_sampler_run(s, 0, nullptr);  // lf.resetStats() after warmup even when no iteration follows (Driver.scala:31)
+  if (rc) return rc;
+  const size_t C = (size_t)chains, n = m->n_params, I = (size_t)cfg->iterations, mo = g->plan.m_out;
+  std::vector<rn_chain_stats> st(C);
+  if (I > 0) {
+    const size_t want[2] = {I * n * C * 8 /* draws [I][n][C] */, C * I * mo * 8 /* predictive draws [C][I][m_out] */};
+    for (int k = 0; k < 2; k++)
+      if (m->pool_bytes[k] < want[k]) {
+        if (m->pool[k]) A->cuMemFree(m->pool[k]);
+        m->pool[k] = 0;
+        m->pool_bytes[k] = 0;
+        CU(A->cuMemAlloc(&m->pool[k], want[k]));
+        m->pool_bytes[k] = want[k];
+      }
+    rc = rn_sampler_run(s, (int)I, (double*)(uintptr_t)m->pool[0]);
+    if (rc) return rc;
+  }
+  rc = rn_sampler_stats(s, st.data(), mass, cfg->stats_rings);  // the sampling streams' final states
+  if (rc) return rc;
+  if (I > 0) {
+    if (cfg->diagnostics) {
+      rc = rn_sampler_diagnostics(s, (const double*)(uintptr_t)m->pool[0], (int)I, 0, cfg->diagnostics);
+      if (rc) return rc;
+    }
+    std::vector<rn_rng_state> rng(C);
+    for (size_t c = 0; c < C; c++) rng[c] = st[c].rng;
+    rc = generator_run(A, g, (const double*)(uintptr_t)m->pool[0], RN_LAYOUT_SAMPLER, (int64_t)I, (int64_t)C, rng.data(),
+                       (double*)(uintptr_t)m->pool[1], s->stream);
+    if (rc) return rc;
+    for (size_t c = 0; c < C; c++) st[c].rng = rng[c];
+    rc = drain_to_host(A, s->stream, m->pool[1], out, C * I * mo * 8, /*sync=*/true);
+    if (rc) return rc;
+  }
+  if (stats) std::memcpy(stats, st.data(), C * sizeof(rn_chain_stats));
+  return RN_OK;
+}
+
+}  // extern "C"

@@ -53,6 +53,19 @@ public final class Native {
 
   public static native void functionDestroy(long handle);
 
+  /** rn_generator_*: Trace.predict's Generator.get on the device for a RIR_FLAG_GENERATOR container.  rng: long[3 * chains] =
+   *  (seed48, doubleToRawLongBits(nextNextGaussian), haveNextNextGaussian) per chain, continued in place */
+  public static native long generatorCreate(ByteBuffer rir, int device);
+
+  public static native int generatorOutputs(long handle);
+
+  public static native void generatorEval(long handle, double[] draws, long iterations, long chains, long[] rng, double[] out);
+
+  public static native void generatorDestroy(long handle);
+
+  /** rn_sample_generate: model.sample(config).predict(gen) with the draws on the device; rngOut as generatorEval's rng */
+  public static native void sampleGenerate(long model, ByteBuffer config, long generator, long[] seeds, double[] out, long[] rngOut);
+
   /** rn_optimize: Optimizer.lbfgs for a batch of starts; x0 == null: every start at 0 (the reference's start) */
   public static native void optimize(long handle, double[] x0, int starts, int m, double eps, int maxEvals, double[] x, int[] info);
 
