@@ -58,6 +58,9 @@ struct RnArgs {
   // the chains' log2 initial step sizes) and step_acc[1] (chains); a warmup launch of one iteration adds its quantised
   // acceptance probabilities into *step_acc (the slot of that iteration)
   rn_i64* step_acc;
+  // warp-per-chain modules with RN_WPC_PLACE > 0 (rn_sampler_wpc.cuh): the chains' state slices that do not fit shared memory,
+  // [chain][RN_WPC_GLOBAL_DOUBLES]; NULL otherwise
+  double* wpc_state;
 };
 
 // argument block of rn_k_eval (rn_function.cuh): batched evaluation of a compiled function, generic addressing
@@ -81,6 +84,8 @@ struct RnOptArgs {
   double eps;         // Optimizer.scala:13
   int starts;
   int max_evals;
+  int pad0;
+  double* wpc_state;  // warp per start with RN_WPC_PLACE > 0 (rn_optimizer.cuh): [start][RN_OPT_GLOBAL_DOUBLES]; NULL otherwise
 };
 
 #endif

@@ -305,14 +305,14 @@ struct Emitter {
         auto ri = row_index.find(sc.index_node);
         if (ri != row_index.end() && ri->second.low == sc.low && ri->second.len == sc.len) {
           // the forward Lookup's index (-1: outside the table, flag already raised there)
-          os << ind << "{ const int k = " << ri->second.var << "; const bool bad = k < 0; rn_scatter_add(&scr["
+          os << ind << "{ const int k = " << ri->second.var << "; const bool bad = k < 0; " << scatter_fn() << "(&scr["
              << (scatter_base_off + smem_slot[sc.slot_base]) << " + (bad ? 0 : k)], bad ? 0.0 : " << val(sc.node) << "); }\n";
           return;
         }
         // branch-free (an index outside the table raises the flag and adds 0 to entry 0) and in the shared state space: the
         // generic atomicAdd carries one code path per address space behind a run-time test, 16 times per row body on cfg 5
         os << ind << "{ const int k = rn_d2i(" << val(sc.index_node) << ") - (" << sc.low << "); const bool bad = (unsigned)k >= " << sc.len
-           << "u; err |= (int)bad; rn_scatter_add(&scr[" << (scatter_base_off + smem_slot[sc.slot_base]) << " + (bad ? 0 : k)], bad ? 0.0 : "
+           << "u; err |= (int)bad; " << scatter_fn() << "(&scr[" << (scatter_base_off + smem_slot[sc.slot_base]) << " + (bad ? 0 : k)], bad ? 0.0 : "
            << val(sc.node) << "); }\n";
         return;
       }
@@ -1608,7 +1608,7 @@ struct Emitter {
         const int m = (int)round_sums.size();
         for (int sidx : round_sums) os << "  s" << sidx << " = rn_warp_sum(s" << sidx << ");\n";
         if (K > 1) {
-          os << "  {\n    double* red = scr + " << red_off << ";\n    const int wg = lane >> 5;\n    RN_SYNC();\n    if ((lane & 31) == 0) {\n";
+          os << "  {\n    double* red = " << red_ptr() << ";\n    const int wg = lane >> 5;\n    RN_SYNC();\n    if ((lane & 31) == 0) {\n";
           for (int j = 0; j < m; j++) os << "      red[wg * " << m << " + " << j << "] = s" << round_sums[j] << ";\n";
           os << "    }\n    RN_SYNC();\n";
           for (int j = 0; j < m; j++) {
@@ -1630,6 +1630,10 @@ struct Emitter {
       }
     }
   }
+
+  // placement 1 (RN_WPC_PLACE): the density scratch is in global memory, its cross-warp reduction slots are not (own argument)
+  std::string red_ptr() const { return opt.wpc_place == 1 ? std::string("red_s") : "scr + " + std::to_string(red_off); }
+  const char* scatter_fn() const { return opt.wpc_place == 1 ? "rn_scatter_add_global" : "rn_scatter_add"; }
 
   void density_wpc() {
     wpc = true;
@@ -1670,7 +1674,7 @@ struct Emitter {
     }
     if (!any_full) mma_all_ok = false;
     if (!mma_all_ok) mma_shared_doubles = 0;
-    const bool use_mma = opt.mma && mma_all_ok;
+    const bool use_mma = opt.mma && mma_all_ok && opt.wpc_place == 0;  // the DMMA path reads q / scratch through shared addresses
     kernel_uses_mma = use_mma;
     int n_reg_acc = 0;
     for (int sl = 0; sl < P.n_slots; sl++)
@@ -1685,6 +1689,8 @@ struct Emitter {
     os << "#define RN_WPC_SCRATCH " << (tab_doubles + n_smem_acc + red_doubles + (use_mma ? (int)mma_inv.size() : 0)) << "\n";
     os << "#define RN_MMA_BARS " << (use_mma ? MMA_WARPS : 0) << "\n";
     os << "#define RN_WPC_RED_OFF " << red_off << "\n";
+    if (opt.wpc_place == 1) os << "#define RN_WPC_RED_DOUBLES " << red_doubles << "\n#define RN_DENSITY_RED(p) , p\n";
+    else os << "#define RN_DENSITY_RED(p)\n";
     os << "RN_DEVICE double rn_tab_lookup(const double* tab, int len, int low, double idx, int& err) {\n"
           "  const int k = rn_d2i(idx) - low;\n  const bool bad = (unsigned)k >= (unsigned)len;\n  err |= (int)bad;\n"
           "  const double v = tab[bad ? 0 : k];\n  return bad ? RN_NAN : v;\n}\n";
@@ -1698,8 +1704,9 @@ struct Emitter {
         if (plans[t].ok)
           for (size_t di = 0; di < (plans[t].uniform ? 1 : plans[t].dots.size()); di++) mma_helper(P.targets[t], t, plans[t], di);
     os << "RN_DEVICE void rn_density(const double* q, double& dens, double* grad, double* scr, "
-          "const double* RN_RESTRICT data, int& err_io, RnTma& tma) {\n";
+       << (opt.wpc_place == 1 ? "double* red_s, " : "") << "const double* RN_RESTRICT data, int& err_io, RnTma& tma) {\n";
     // the error flag in a register: through the reference it lived in local memory, one LDL / LOP3 / STL chain per lookup
+    if (opt.wpc_place == 1) os << "  (void)red_s;\n";
     os << "  (void)data; (void)scr; (void)tma;\n  const int lane = (int)(threadIdx.x % RN_G);  // thread of the chain's group\n  (void)lane;\n"
        << "  int err = 0;\n";
     if (n_smem_acc) os << "  for (int k = lane; k < " << n_smem_acc << "; k += RN_G) scr[" << tab_doubles << " + k] = 0.0;\n";
@@ -1772,7 +1779,7 @@ struct Emitter {
       // the K warps of the chain exchange their partial sums through shared memory; every thread adds them in the same
       // order, so all of them hold identical totals afterwards
       const int stride = n_reg_acc + 1;
-      os << "  {\n    double* red = scr + " << red_off << ";\n    const int wg = lane >> 5;\n    if ((lane & 31) == 0) {\n";
+      os << "  {\n    double* red = " << red_ptr() << ";\n    const int wg = lane >> 5;\n    if ((lane & 31) == 0) {\n";
       int idx = 0;
       for (int sl = 0; sl < P.n_slots; sl++)
         if (smem_slot[sl] < 0) os << "      red[wg * " << stride << " + " << idx++ << "] = a" << sl << ";\n";
@@ -1823,8 +1830,16 @@ WpcSizes wpc_sizes(const Program& P, const EmitOptions& opt) {
   Emitter E(P, opt);
   E.density_wpc();
   // chain vectors (q, p, gradient, mass [+ EHMC snapshot]) [+ 2 scratch vectors of the dense mass matrix code] + density scratch
-  z.scratch_doubles = E.tab_doubles + E.n_smem_acc + E.red_doubles + ((opt.mma && E.mma_all_ok) ? (int)E.mma_inv.size() : 0);
-  z.per_warp_doubles = wpc_vectors(opt) * (int)P.n_params + z.scratch_doubles;
+  z.scratch_doubles = E.tab_doubles + E.n_smem_acc + E.red_doubles + ((opt.mma && E.mma_all_ok && opt.wpc_place == 0) ? (int)E.mma_inv.size() : 0);
+  z.vector_doubles = wpc_vectors(opt) * (int)P.n_params;
+  z.red_doubles = E.red_doubles;
+  const long long vec = z.vector_doubles, scr = z.scratch_doubles;
+  if (opt.wpc_place == 0) {  // rn_sampler_wpc.cuh: RN_WPC_SMEM_DOUBLES / RN_WPC_GLOBAL_DOUBLES
+    z.per_warp_doubles = (int)(vec + scr);
+  } else {
+    z.per_warp_doubles = z.red_doubles;
+    z.global_doubles = (vec + scr + 15) / 16 * 16;
+  }
   for (const TargetInfo& T : P.targets)
     if (T.streamed() && T.n_rows >= 32ull * (uint64_t)std::max(1, opt.wpc_k))
       z.tile_doubles = std::max(z.tile_doubles, (int)T.n_cols * opt.pitch((size_t)(&T - &P.targets[0])) * std::max(1, opt.wpc_k));
@@ -1849,6 +1864,8 @@ std::string emit_optimizer_source(const Program& P, const EmitOptions& opt, int 
   os << "#define RN_BACKEND " << (opt.backend == 1 ? 1 : 0) << "\n";
   os << "#define RN_LBFGS_M " << history << "\n";
   if (opt.expect_slice_doubles > 0) os << "#define RN_OPT_EXPECT_SMEM " << opt.expect_slice_doubles << "\n";
+  if (opt.expect_global_doubles >= 0) os << "#define RN_OPT_EXPECT_GLOBAL " << opt.expect_global_doubles << "\n";
+  if (opt.backend == 1) os << "#define RN_WPC_PLACE " << opt.wpc_place << "\n";
   if (opt.fast_math) os << "#define RN_FAST_MATH 1\n";
   EmitOptions eo = opt;
   if (opt.backend == 1) {  // K warps per start, independent per-warp row loads (no CTA-shared tiles: starts diverge)
@@ -1955,6 +1972,9 @@ std::string emit_source(const Program& P, const EmitOptions& opt) {
   if (opt.backend == 0) os << "#define RN_TS_RESTORE " << (opt.tpc_restore ? 1 : 0) << "\n";
   if (opt.backend == 1) {
     os << "#define RN_WPC_K " << std::max(1, opt.wpc_k) << "\n";
+    os << "#define RN_WPC_PLACE " << opt.wpc_place << "\n";
+    if (opt.expect_slice_doubles > 0) os << "#define RN_WPC_EXPECT_SMEM " << opt.expect_slice_doubles << "\n";
+    if (opt.expect_global_doubles >= 0) os << "#define RN_WPC_EXPECT_GLOBAL " << opt.expect_global_doubles << "\n";
     os << "#define RN_TMA_STAGES " << opt.tma_stages << "\n";
     {
       const WpcSizes z = wpc_sizes(P, opt);
@@ -1962,8 +1982,14 @@ std::string emit_source(const Program& P, const EmitOptions& opt) {
     }
   }
   os << kPreludeSource << "\n" << kSamplerCommonSource << "\n";
-  if (opt.backend == 1)  // (RN_WPC_SCRATCH is defined by the emitted density; macros expand where they are used)
-    os << "#define RN_WPC_SMEM_DOUBLES (" << wpc_vectors(opt) << " * RN_N + RN_WPC_SCRATCH)\n";
+  if (opt.backend == 1) {  // (RN_WPC_SCRATCH is defined by the emitted density; macros expand where they are used)
+    const int v = wpc_vectors(opt);
+    if (opt.wpc_place == 0)
+      os << "#define RN_WPC_SMEM_DOUBLES (" << v << " * RN_N + RN_WPC_SCRATCH)\n#define RN_WPC_GLOBAL_DOUBLES 0\n";
+    else
+      os << "#define RN_WPC_SMEM_DOUBLES (RN_WPC_RED_DOUBLES)\n#define RN_WPC_GLOBAL_DOUBLES ((" << v
+         << "LL * RN_N + RN_WPC_SCRATCH + 15) / 16 * 16)\n";
+  }
   os << emit_density(P, opt) << "\n";
   if (opt.backend == 1) {
     os << kSamplerWpcSource << "\n";

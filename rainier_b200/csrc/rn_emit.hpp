@@ -18,12 +18,15 @@ struct EmitOptions {
   bool tpc_restore = false; // thread per chain: the iteration's restore point in shared memory (RN_TS_RESTORE, rn_sampler.cuh)
   int tma_stages = 0;     // warp per chain: shared-memory stages of the CTA-shared data-tile pipeline (0 = off)
   int wpc_k = 1;          // warp per chain: warps owning one chain (1, 2, 4 or 8; > 1 for chains with a large state)
+  int wpc_place = 0;      // warp per chain: where a chain's state lives (RN_WPC_PLACE): 0 all in shared memory, 1 the chain
+                          // vectors and the density scratch in global memory (the reduction slots stay in shared memory)
   std::vector<uint64_t> target_base;  // per target: element offset of its tile-major [tile][column][pitch] block in the data buffer
   std::vector<int> target_pitch;      // per target: doubles between consecutive columns of a tile (32 rows + padding; empty = 32).
                                       // 36 where the chain-batched DMMA path may run: X^T fragments are then bank-conflict free
   bool mma = false;       // warp per chain: chain-batched fp64 tensor-core contraction of the row bodies' dot products (see
                           // Emitter::mma_block); needs full CTAs of mma_chains chains (= warps, wpc_k == 1)
-  int expect_slice_doubles = 0;  // optimizer: the launcher's shared-memory doubles per start (checked against the kernel's own layout at compile time)
+  int expect_slice_doubles = 0;  // the launcher's shared-memory doubles per chain / start (checked against the kernel's own layout at compile time)
+  long long expect_global_doubles = -1;  // the launcher's global-memory state doubles per chain / start (likewise; -1 = unchecked)
   int interleave = 8;     // independent dataflow components of a row body (unrolled observations) emitted round-robin at a time
   int mma_chains = 8;     // 8 or 16: chains (warps) per CTA on that path -- 16 = two groups of 8 chains whose warps pair up on
                           // a dot's column block (twice the warps per SM for the same shared memory)
@@ -48,8 +51,12 @@ std::string emit_optimizer_source(const Program& P, const EmitOptions& opt, int 
 // shared-memory needs of the warp-per-chain kernels: doubles per warp (chain vectors + density scratch) and doubles of
 // the largest data tile (n_cols * 32 over the streamed targets; 0 when nothing is streamed)
 struct WpcSizes {
-  int per_warp_doubles = 0;  // per CHAIN (its wpc_k warps share the slice): the sampler's vectors + scratch_doubles
+  int per_warp_doubles = 0;  // per CHAIN (its wpc_k warps share the slice), shared memory in placement opt.wpc_place:
+                             // 0 vector_doubles + scratch_doubles, 1 red_doubles
+  long long global_doubles = 0;  // per chain in global memory (RN_WPC_GLOBAL_DOUBLES): 0, or vectors + scratch; 128-byte multiple
+  int vector_doubles = 0;    // the sampler's chain vectors (q, p, gradient, mass, EHMC snapshot, dense work vectors)
   int scratch_doubles = 0;   // the emitted density's part of it (RN_WPC_SCRATCH): tables, scatter slots, reduction scratch
+  int red_doubles = 0;       // the cross-warp reduction slots inside that scratch (RN_WPC_RED_DOUBLES; 0 when wpc_k == 1)
   int tile_doubles = 0;
   bool mma_ok = false;       // every streamed target with full tiles can take the chain-batched DMMA path
   int mma_shared_doubles = 0;  // CTA-shared doubles of that path: 8 per-warp column-block regions + the reduction scratch

@@ -371,13 +371,27 @@ RN_DEVICE int rn_lb_apply(RnLbfgs& S, const double f, const double* g) {
 // at x, info [starts] (bit 0 evaluation cap reached, bit 1 "dginit", bit 2 lookup error), evals [starts]
 // =============================================================================================================
 #if RN_BACKEND == 1
-// shared-memory slice of one start: x | gradient | g = -gradient | diag | w | scratch of the emitted density | K reduction slots
+// slices of one start, by placement (RN_WPC_PLACE, as for the samplers: rn_sampler_wpc.cuh):
+//   0  shared: x | gradient | g = -gradient | diag | w | scratch of the emitted density | K reduction slots
+//   1  global: x | gradient | g | diag | w | density scratch  shared: K reduction slots | the density's reduction slots
+#if RN_WPC_PLACE == 0
 #define RN_OPT_SMEM_DOUBLES (4 * RN_N + RN_LB_W + RN_WPC_SCRATCH + RN_WPC_K)
+#define RN_OPT_GLOBAL_DOUBLES 0
+#else
+#define RN_OPT_SMEM_DOUBLES (RN_WPC_K + RN_WPC_RED_DOUBLES)
+#define RN_OPT_GLOBAL_DOUBLES ((4LL * RN_N + RN_LB_W + RN_WPC_SCRATCH + 15) / 16 * 16)
+#endif
 #ifdef RN_OPT_EXPECT_SMEM  // what rn_runtime.cpp:get_opt_kernel allocates per start; a mismatch is a slice overrun on the device
 static_assert(RN_OPT_SMEM_DOUBLES == RN_OPT_EXPECT_SMEM, "rn_optimize: launcher and kernel disagree on the shared-memory slice of a start");
 #endif
+#ifdef RN_OPT_EXPECT_GLOBAL
+static_assert(RN_OPT_GLOBAL_DOUBLES == RN_OPT_EXPECT_GLOBAL, "rn_optimize: launcher and kernel disagree on the global-memory slice of a start");
+#endif
 #ifdef RN_HOST_EMULATION
 static double rn_smem[1 << 17];  // one emulated start at a time
+#if RN_WPC_PLACE != 0  // ... with its global slice here (tests/host_emulation.py passes no slice array)
+static double rn_emu_wpc_state[(size_t)RN_OPT_GLOBAL_DOUBLES * 8];
+#endif
 #else
 extern __shared__ __align__(128) double rn_smem[];
 #endif
@@ -387,10 +401,21 @@ RN_GLOBAL void rn_k_lbfgs(const RnOptArgs A) {
 #if RN_BACKEND == 1
   const int c = (int)((blockIdx.x * blockDim.x + threadIdx.x) / RN_G);
   if (c >= A.starts) return;  // the whole group leaves together
-  double* base = rn_smem + (size_t)RN_GROUP * RN_OPT_SMEM_DOUBLES;
-  double *x = base, *grad = base + RN_N, *g = base + 2 * RN_N, *diag = base + 3 * RN_N, *w = base + 4 * RN_N;
+  double* sbase = rn_smem + (size_t)RN_GROUP * RN_OPT_SMEM_DOUBLES;
+#if RN_WPC_PLACE == 0
+  double* base = sbase;
   double* scr = base + 4 * RN_N + RN_LB_W;
   double* red = scr + RN_WPC_SCRATCH;
+#else
+#ifdef RN_HOST_EMULATION
+  double* base = rn_emu_wpc_state + (size_t)RN_GROUP * (size_t)RN_OPT_GLOBAL_DOUBLES;
+#else
+  double* base = A.wpc_state + (size_t)c * (size_t)RN_OPT_GLOBAL_DOUBLES;
+#endif
+  double* scr = base + 4 * RN_N + RN_LB_W;
+  double* red = sbase;
+#endif
+  double *x = base, *grad = base + RN_N, *g = base + 2 * RN_N, *diag = base + 3 * RN_N, *w = base + 4 * RN_N;
   RnTma tma;  // the CTA-shared tile pipeline stays off: starts take different numbers of evaluations
   tma.on = 0;
   tma.seq = 0;
@@ -416,7 +441,7 @@ RN_GLOBAL void rn_k_lbfgs(const RnOptArgs A) {
     double dens;
     RN_LB_SYNC();  // x was written lane-strided; the density reads all of it in every lane
 #if RN_BACKEND == 1
-    rn_density(x, dens, grad, scr, A.data, err, tma);  // df.update(x), Optimizer.scala:15 (ends with a group barrier)
+    rn_density(x, dens, grad, scr RN_DENSITY_RED(red + RN_WPC_K), A.data, err, tma);  // df.update(x), Optimizer.scala:15 (ends with a group barrier)
 #else
     rn_density(S_X_ARRAY(x), dens, S_X_ARRAY(grad), A.data, err);  // df.update(x), Optimizer.scala:15
 #endif

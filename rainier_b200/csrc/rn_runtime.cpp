@@ -81,6 +81,7 @@ const Api* api(std::string* why) {
       RN_SYM(cuModuleGetFunction, "cuModuleGetFunction")
       RN_SYM(cuMemAlloc, "cuMemAlloc_v2")
       RN_SYM(cuMemFree, "cuMemFree_v2")
+      RN_SYM(cuMemGetInfo, "cuMemGetInfo_v2")
       RN_SYM(cuMemAllocHost, "cuMemAllocHost_v2")
       RN_SYM(cuMemFreeHost, "cuMemFreeHost")
       RN_SYM(cuMemHostRegister, "cuMemHostRegister_v2")
@@ -208,6 +209,8 @@ struct Kernel {
   bool mass_pool = false;     // rn_k_pool_reduce_dense / rn_k_pool_factor / rn_k_pool_apply_dense compiled in (pooled dense windows)
   unsigned tpc_block = 0;     // backend 0: the CTA size this module was compiled for (0: reads blockDim.x)
   int wpc_smem_doubles = 0;   // per-warp dynamic shared memory (backend 1)
+  int wpc_place = 0;          // backend 1: RN_WPC_PLACE, where a chain's state lives (rn_sampler_wpc.cuh)
+  long long wpc_global_doubles = 0;  // backend 1: per-chain slice of the global state array (RnArgs::wpc_state), 0 in placement 0
   int warps_per_cta = 4;      // backend 1: CHAINS per CTA (each owned by wpc_k warps)
   int wpc_k = 1;
   int tma_stages = 0;         // CTA-shared data-tile pipeline (backend 1): stages, doubles per stage
@@ -261,6 +264,7 @@ struct rn_model {
     int smem_doubles = 0;      // backend 1: shared-memory slice of one start
     int starts_per_cta = 1;    // backend 1
     int wpc_k = 1;             // backend 1: warps per start
+    long long global_doubles = 0;  // backend 1: per-start slice of the global state array (RnOptArgs::wpc_state)
   };
   std::map<std::tuple<bool, bool, int, int>, std::unique_ptr<OptKernel>> opt_kernels;
 };
@@ -315,6 +319,58 @@ static KernelKey key_for(const rn_model* m, const rn_config* cfg) {
   return k;
 }
 
+// Placement of the per-chain (per-start) state of the warp-per-chain kernels and the warps per chain, decided in one place for
+// the samplers and the optimizer.  shared_doubles(place, k): shared-memory doubles one chain needs in placement `place`
+// (RN_WPC_PLACE: 0 all state, 1 only the reduction slots; the rest goes to global memory) with k warps.  The lowest placement
+// whose slice fits `cap` bytes is taken, so a model that fits shared memory stays on placement 0.  (An intermediate placement
+// that kept the density scratch in shared memory was measured slower than placement 1 on the model it would have served:
+// DESIGN.md 3.2b.)
+// Warps per chain: one, unless so few chains fit an SM beside `reserve` bytes of data tiles that it would hold fewer than 16
+// warps.  RN_WPC_PLACE (tests) forces a higher placement; a lower one than the sizes allow is refused, as is RN_WPC_K.
+static int wpc_place(const std::function<uint64_t(int, int)>& shared_doubles, uint64_t cap, uint64_t reserve, const char* what,
+                     int* place_out, int* k_out) {
+  int place = 0;
+  while (place <= 1 && shared_doubles(place, 1) * 8 > cap) place++;
+  if (place > 1) return fail(RN_E_UNSUPPORTED, what);
+  if (const char* e = getenv("RN_WPC_PLACE")) {
+    const int want = atoi(e);
+    if (want < place)
+      return fail(RN_E_INVALID, "RN_WPC_PLACE=" + std::to_string(want) + ": the per-chain state needs placement " + std::to_string(place));
+    place = std::min(1, want);
+  }
+  for (;; place++) {
+    if (place > 1) return fail(RN_E_UNSUPPORTED, what);
+    const uint64_t one = std::max<uint64_t>(8, shared_doubles(place, 1) * 8);
+    if (one > cap) continue;
+    const uint64_t fit = std::max<uint64_t>(1, (cap - std::min<uint64_t>(cap / 4, reserve)) / one);
+    int k = 1;
+    while (k < 8 && fit * (uint64_t)k < 16) k *= 2;  // aim at 16 warps per SM (cfg 5 gains with each doubling of K)
+    if (const char* e = getenv("RN_WPC_K")) k = std::max(1, std::min(8, atoi(e)));
+    if (k != 1 && k != 2 && k != 4 && k != 8) k = 1;
+    if (shared_doubles(place, k) * 8 > cap) continue;  // the reduction slots of k warps tip it over: next placement
+    *place_out = place;
+    *k_out = k;
+    return RN_OK;
+  }
+}
+
+// The global slice array of placements 1 and 2 ([count][per_chain_doubles], 128-byte aligned slices): checked against the
+// device's free memory first, so that too many chains fail here, with the sizes, instead of inside a launch.  *out stays 0 in
+// placement 0.
+static int alloc_state_slices(const Api* A, size_t count, long long per_chain_doubles, const char* who, CUdeviceptr* out) {
+  *out = 0;
+  if (per_chain_doubles <= 0) return RN_OK;
+  const size_t bytes = count * (size_t)per_chain_doubles * 8;
+  size_t free_bytes = 0, total_bytes = 0;
+  CU(A->cuMemGetInfo(&free_bytes, &total_bytes));
+  if (bytes > free_bytes)
+    return fail(RN_E_CUDA, std::string(who) + ": the state that does not fit shared memory needs " + std::to_string(bytes) +
+                               " bytes of device memory for " + std::to_string(count) + " chains (" + std::to_string(free_bytes) +
+                               " free); use fewer chains");
+  CU(A->cuMemAlloc(out, bytes));
+  return RN_OK;
+}
+
 extern "C" const char* rn_version(void);
 // emit + NVRTC (no device needed)
 // source_only: just emit (rn_emit_source, the analogue of rainier-decompile) -- no NVRTC run, nothing cached
@@ -363,24 +419,32 @@ static int get_kernel(rn_model* m, const rn_config* cfg, Kernel** out, std::stri
                                          // shared memory and the 1 KB the system reserves per CTA is outside that figure)
     int wmax = 8;
     if (const char* e = getenv("RN_WPC_WARPS")) wmax = std::max(1, std::min(32, atoi(e)));
-    // warps per chain: one, unless the chain's shared-memory state is so large that fewer than 16 chains fit an SM
+    // placement of the chain's state and warps per chain (wpc_place); the sizes of one emitter pass serve every placement
     {
-      const WpcSizes z1 = wpc_sizes(*P, eo);
-      const size_t pc = (size_t)z1.per_warp_doubles * 8;
-      if (pc > cap) return fail(RN_E_UNSUPPORTED, "model state does not fit one chain's shared memory slice");
-      const size_t fit = std::max<size_t>(1, (cap - std::min<size_t>(cap / 4, 2 * (size_t)z1.tile_doubles * 8)) / pc);
-      int k = 1;
-      while (k < 8 && fit * (size_t)k < 16) k *= 2;  // aim at 16 warps per SM (cfg 5 gains with each doubling of K)
-      if (const char* e = getenv("RN_WPC_K")) k = std::max(1, std::min(8, atoi(e)));
-      if (k != 1 && k != 2 && k != 4 && k != 8) k = 1;
+      std::map<int, WpcSizes> by_k;
+      auto shared = [&](int place, int k) -> uint64_t {
+        auto it = by_k.find(k);
+        if (it == by_k.end()) {
+          EmitOptions e = eo;
+          e.wpc_k = k;
+          it = by_k.emplace(k, wpc_sizes(*P, e)).first;
+        }
+        const WpcSizes& z = it->second;
+        return place == 0 ? (uint64_t)z.vector_doubles + z.scratch_doubles : (uint64_t)z.red_doubles;
+      };
+      int place = 0, k = 1;
+      rc = wpc_place(shared, cap, 2 * (uint64_t)wpc_sizes(*P, eo).tile_doubles * 8, "model state does not fit one chain's shared memory slice",
+                     &place, &k);
+      if (rc) return rc;
+      eo.wpc_place = K->wpc_place = place;
       eo.wpc_k = K->wpc_k = k;
     }
     if (eo.wpc_k > 1) wmax = std::min(wmax, 14);  // named barriers 2..15, one per chain slot
     const WpcSizes z = wpc_sizes(*P, eo);
     K->wpc_smem_doubles = z.per_warp_doubles;
+    K->wpc_global_doubles = z.global_doubles;
     K->tile_doubles = z.tile_doubles;
     const size_t per_warp = (size_t)z.per_warp_doubles * 8, tile = (size_t)z.tile_doubles * 8;
-    if (per_warp > cap) return fail(RN_E_UNSUPPORTED, "model state does not fit one chain's shared memory slice");
     // data-tile stages: two (prefetch overlaps compute) when at least 4 chains still fit beside them, else one, else off
     int stages = 0;
     if (tile > 0) {
@@ -399,7 +463,7 @@ static int get_kernel(rn_model* m, const rn_config* cfg, Kernel** out, std::stri
     eo.tma_stages = stages;
     // chain-batched fp64 tensor-core path (rn_emit.cpp: Emitter::mma_block): HMC (every chain of a CTA evaluates the density
     // equally often), not the dense-mass code, one warp per chain, 8 chains per CTA, and every streamed target eligible
-    bool want_mma = !key.ehmc && key.mass_max < 2 && eo.wpc_k == 1 && z.mma_ok && !P->symbolic;
+    bool want_mma = !key.ehmc && key.mass_max < 2 && eo.wpc_k == 1 && eo.wpc_place == 0 && z.mma_ok && !P->symbolic;
     if (const char* e = getenv("RN_MMA")) want_mma = want_mma && atoi(e) != 0;
     if (want_mma) {
       // 16 chains per CTA when they fit (two chain groups whose warps pair up on a dot's column block: twice the warps per
@@ -424,6 +488,8 @@ static int get_kernel(rn_model* m, const rn_config* cfg, Kernel** out, std::stri
         }
       }
     }
+    eo.expect_slice_doubles = K->wpc_smem_doubles;
+    eo.expect_global_doubles = K->wpc_global_doubles;
   }
   if (eo.backend == 1) {  // registers per thread the CTA leaves (see the cap below): fewer components in flight when it is tight
     const int warps = K->warps_per_cta * K->wpc_k;
@@ -922,17 +988,21 @@ int rn_density_batch(rn_model* m, const double* q, int chains, double* out) {
   std::vector<double> qt((size_t)n * chains), ot((size_t)(n + 1) * chains);
   for (int c = 0; c < chains; c++)
     for (int i = 0; i < n; i++) qt[(size_t)i * chains + c] = q[(size_t)c * n + i];
-  CUdeviceptr dq = 0, dout = 0, derr = 0;
+  CUdeviceptr dq = 0, dout = 0, derr = 0, dstate = 0;
   struct Free {  // released on every exit path
     const Api* A;
-    CUdeviceptr *a, *b, *c;
+    CUdeviceptr *a, *b, *c, *d;
     ~Free() {
-      for (CUdeviceptr* p : {a, b, c})
+      for (CUdeviceptr* p : {a, b, c, d})
         if (*p) A->cuMemFree(*p);
     }
-  } guard{A, &dq, &dout, &derr};
+  } guard{A, &dq, &dout, &derr, &dstate};
   rc = make_current(A, m);
   if (rc) return rc;
+  if (K->backend == 1) {
+    rc = alloc_state_slices(A, (size_t)chains, K->wpc_global_doubles, "rn_density_batch", &dstate);
+    if (rc) return rc;
+  }
   CU(A->cuMemAlloc(&dq, qt.size() * 8 + 8));
   CU(A->cuMemAlloc(&dout, ot.size() * 8));
   CU(A->cuMemAlloc(&derr, 4));
@@ -940,7 +1010,7 @@ int rn_density_batch(rn_model* m, const double* q, int chains, double* out) {
   CU(A->cuMemcpyHtoD(dq, qt.data(), qt.size() * 8));
   CUdeviceptr ddata = m->d_data;
   int ch = chains;
-  void* params[] = {&dq, &dout, &ddata, &derr, &ch};
+  void* params[] = {&dq, &dout, &ddata, &derr, &ch, &dstate};  // (the thread-per-chain rn_k_density takes the first five)
   if (K->backend == 1) {
     const unsigned w = (unsigned)K->warps_per_cta;
     CU(A->cuLaunchKernel(K->k_density, (unsigned)((chains + w - 1) / w), 1, 1, w * 32 * (unsigned)K->wpc_k, 1, 1,
@@ -1031,6 +1101,7 @@ struct rn_sampler {
   CUdeviceptr d_trace = 0;  // optional test instrumentation, [warmup+iterations][4][chains]
   size_t trace_iters = 0, trace_pos = 0;
   rn_comm* comm = nullptr;
+  CUdeviceptr d_state = 0;  // warp per chain, RN_WPC_PLACE > 0: the chains' global state slices (RnArgs::wpc_state)
   CUdeviceptr d_pool = 0;  // pooled window statistics (RN_ADAPT_POOLED): [2n+1], dense [1+n+n^2] + factor scratch
   CUdeviceptr d_step = 0;  // int64 [2 + warmup]: K, C, Q_t of pooled step-size adaptation (rn_sampler_common.cuh), zeroed at create
   // device time of the sampling phase (Stats.gradientTimes / iterationTimes, Stats.scala:8-9): events bracket every
@@ -1239,9 +1310,14 @@ int rn_sampler_create(rn_model* m, const rn_config* cfg, const int64_t* seeds, i
   }
   s->d_pool = s->arena + pool_off;  // the pooled window statistics live behind the chain state
   CU(A->cuMemsetD8Async(s->arena, 0, s->arena_bytes, s->stream));
+  if (s->K->backend == 1) {
+    rc = alloc_state_slices(A, C, s->K->wpc_global_doubles, "rn_sampler_create", &s->d_state);
+    if (rc) return rc;
+  }
 
   RnArgs& a = s->args;
   std::memset(&a, 0, sizeof(a));
+  a.wpc_state = (double*)(uintptr_t)s->d_state;
   auto P = [&](size_t o) { return (void*)(uintptr_t)(s->arena + o); };
   a.chains = chains;
   a.params = (double*)P(o_params);
@@ -2013,6 +2089,7 @@ void rn_sampler_destroy(rn_sampler* s) {
       }
     }
     if (s->d_trace) A->cuMemFree(s->d_trace);
+    if (s->d_state) A->cuMemFree(s->d_state);
     if (s->d_track) A->cuMemFree(s->d_track);
     if (s->d_track_terms) A->cuMemFree(s->d_track_terms);
     if (s->d_track_sums) A->cuMemFree(s->d_track_sums);
@@ -2934,25 +3011,34 @@ static int get_opt_kernel(rn_model* m, const rn_optimize_config* oc, rn_model::O
     eo.tma_stages = 0;
     eo.enable_ehmc = false;
     const uint64_t cap = (227 * 1024 - 2048) / 8;
-    // warps per start: one, unless the start's shared-memory state is so large that fewer than 16 starts fit an SM (same
-    // rule as the samplers, rn_runtime.cpp:get_kernel)
-    int k = 1;
-    {
-      eo.wpc_k = 1;
-      const uint64_t one = 4ull * P->n_params + (uint64_t)wpc_sizes(*P, eo).scratch_doubles + lb_w + 1;
-      if (one > cap) return fail(RN_E_UNSUPPORTED, "rn_optimize: the L-BFGS history of one start does not fit shared memory");
-      const uint64_t fit = std::max<uint64_t>(1, cap / one);
-      while (k < 8 && fit * (uint64_t)k < 16) k *= 2;
-      if (const char* e = getenv("RN_WPC_K")) k = std::max(1, std::min(8, atoi(e)));
-      if (k != 1 && k != 2 && k != 4 && k != 8) k = 1;
-    }
+    // placement of the start's state and warps per start: the samplers' rule (wpc_place)
+    const uint64_t vec = 4ull * P->n_params + lb_w;  // x, gradient, g, diag, history
+    std::map<int, WpcSizes> by_k;
+    auto sizes = [&](int k) -> const WpcSizes& {
+      auto it = by_k.find(k);
+      if (it == by_k.end()) {
+        EmitOptions e = eo;
+        e.wpc_k = k;
+        it = by_k.emplace(k, wpc_sizes(*P, e)).first;
+      }
+      return it->second;
+    };
+    // RN_OPT_SMEM_DOUBLES (rn_optimizer.cuh)
+    auto shared = [&](int place, int k) -> uint64_t {
+      const WpcSizes& z = sizes(k);
+      return (uint64_t)k + (place == 0 ? vec + z.scratch_doubles : (uint64_t)z.red_doubles);
+    };
+    int place = 0, k = 1;
+    rc = wpc_place(shared, cap * 8, 0, "rn_optimize: the L-BFGS history of one start does not fit shared memory", &place, &k);
+    if (rc) return rc;
+    eo.wpc_place = place;
     eo.wpc_k = k;
-    const WpcSizes z = wpc_sizes(*P, eo);  // RN_OPT_SMEM_DOUBLES (rn_optimizer.cuh): 4n (x, gradient, g, diag) + history + density scratch + k
-    const uint64_t per_start = 4ull * P->n_params + (uint64_t)z.scratch_doubles + lb_w + (uint64_t)k;
-    if (per_start > cap) return fail(RN_E_UNSUPPORTED, "rn_optimize: the L-BFGS history of one start does not fit shared memory");
+    const uint64_t per_start = shared(place, k);
     K->wpc_k = k;
     K->smem_doubles = (int)per_start;
+    K->global_doubles = place == 0 ? 0 : (long long)((vec + (uint64_t)sizes(k).scratch_doubles + 15) / 16 * 16);
     eo.expect_slice_doubles = (int)per_start;
+    eo.expect_global_doubles = K->global_doubles;
     // at most 256 threads per CTA (255 registers each fit the register file); named barriers 2..15 when K > 1
     K->starts_per_cta = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)(8 / k), cap / per_start));
   }
@@ -3026,14 +3112,19 @@ int rn_optimize(rn_model* m, const rn_optimize_config* oc, const double* x0, int
   // one allocation: x0 | x | f | info | evals
   const size_t off_x = n * S * 8, off_f = 2 * n * S * 8, off_info = off_f + S * 8, off_ev = off_info + S * 4;
   const size_t total = off_ev + S * 4;
-  CUdeviceptr d = 0;
+  CUdeviceptr d = 0, dstate = 0;
   struct Free {
     const Api* A;
-    CUdeviceptr* p;
+    CUdeviceptr *p, *q;
     ~Free() {
-      if (*p) A->cuMemFree(*p);
+      for (CUdeviceptr* x : {p, q})
+        if (*x) A->cuMemFree(*x);
     }
-  } guard{A, &d};
+  } guard{A, &d, &dstate};
+  if (K->backend == 1) {
+    rc = alloc_state_slices(A, S, K->global_doubles, "rn_optimize", &dstate);
+    if (rc) return rc;
+  }
   CU(A->cuMemAlloc(&d, total + 16));
   std::vector<double> t(n * S);
   if (x0) {
@@ -3052,6 +3143,7 @@ int rn_optimize(rn_model* m, const rn_optimize_config* oc, const double* x0, int
   a.eps = oc ? oc->eps : 0.1;
   a.starts = starts;
   a.max_evals = oc && oc->max_evaluations > 0 ? oc->max_evaluations : 10000;
+  a.wpc_state = (double*)(uintptr_t)dstate;
   void* params[] = {&a};
   if (K->backend == 1) {
     const unsigned spc = (unsigned)K->starts_per_cta;

@@ -39,7 +39,28 @@ struct RnStats {
 // cp.async.bulk (TMA, completion on an mbarrier) while all warps consume tile t from shared memory, so a tile crosses
 // L2 -> SM once per CTA instead of once per chain.  EHMC (per-chain trajectory lengths) and the init kernel keep the
 // independent per-warp path (__ldg from L2/L1).  struct RnTma and the mbarrier / bulk-copy helpers live in rn_prelude.cuh.
-// per-warp shared-memory slice
+// Where a chain's state lives (RN_WPC_PLACE, chosen by rn_runtime.cpp:wpc_place from the sizes): 0 all of it in the chain's
+// shared-memory slice; 1 the chain vectors (q, p, gradient, mass, EHMC snapshot, dense work vectors) and the density scratch in
+// the chain's slice of RnArgs::wpc_state in global memory, with only the cross-warp reduction slots left in shared memory.  The
+// global slices are chain-major and 128-byte aligned, so the lane-strided loops over a vector stay coalesced.
+// A slice carries nothing from one launch to the next (every launch reloads q, p, gradient and mass from RnArgs), so the host
+// emulation (tests/host_emulation.py), which runs one CTA at a time and passes no slice array, keeps the slices of one
+// emulated CTA's chains in a static array of its own.
+#if RN_WPC_PLACE == 0
+#define RN_WPC_GSLICE(state, c) ((double*)nullptr)
+#elif defined(RN_HOST_EMULATION)
+static double rn_emu_wpc_state[(size_t)RN_WPC_GLOBAL_DOUBLES * 32];  // up to 32 chains per emulated CTA
+#define RN_WPC_GSLICE(state, c) (rn_emu_wpc_state + (size_t)RN_GROUP * (size_t)RN_WPC_GLOBAL_DOUBLES)
+#else
+#define RN_WPC_GSLICE(state, c) ((state) + (size_t)(c) * (size_t)RN_WPC_GLOBAL_DOUBLES)
+#endif
+#ifdef RN_WPC_EXPECT_SMEM  // what rn_runtime.cpp:get_kernel allocates per chain; a mismatch is a slice overrun on the device
+static_assert(RN_WPC_SMEM_DOUBLES == RN_WPC_EXPECT_SMEM, "launcher and kernel disagree on the shared-memory slice of a chain");
+#endif
+#ifdef RN_WPC_EXPECT_GLOBAL
+static_assert(RN_WPC_GLOBAL_DOUBLES == RN_WPC_EXPECT_GLOBAL, "launcher and kernel disagree on the global-memory slice of a chain");
+#endif
+// per-chain state
 struct RnW {
   double* q;   // pqBuf.q
   double* p;   // pqBuf.p
@@ -49,6 +70,7 @@ struct RnW {
   double* sp;
   double* sg;
   double* scr;  // emitted density scratch (lookup tables, scatter accumulators)
+  double* red;  // its cross-warp reduction slots (RN_WPC_K doubles and more; shared memory in every placement)
 #if RN_MASS_MAX >= 2
   double* v;    // dense mass: velocity M^-1 p / oldDiff of the covariance estimator
   double* v2;   //             newDiff
@@ -61,12 +83,19 @@ struct RnW {
   RnTma tma;    // shared data-tile pipeline of the CTA (off unless the kernel enables it)
 };
 
-RN_DEVICE void rn_w_setup(RnW& w, double* base) {
+// sbase: the chain's shared-memory slice (RN_WPC_SMEM_DOUBLES); gbase: its global-memory slice (RN_WPC_GLOBAL_DOUBLES)
+RN_DEVICE void rn_w_setup(RnW& w, double* sbase, double* gbase) {
   w.tma.on = 0;
   w.tma.seq = 0;
   w.tma.nthreads = 0;
   w.tma.stage = nullptr;
   w.tma.full = nullptr;
+#if RN_WPC_PLACE == 0
+  (void)gbase;
+  double* const base = sbase;
+#else
+  double* const base = gbase;
+#endif
   w.q = base;
   w.p = base + RN_N;
   w.g = base + 2 * RN_N;
@@ -95,6 +124,11 @@ RN_DEVICE void rn_w_setup(RnW& w, double* base) {
   w.M = nullptr;
   w.chol = nullptr;
   w.ld = 0;
+#endif
+#if RN_WPC_PLACE == 1
+  w.red = sbase;
+#else
+  w.red = w.scr + RN_WPC_RED_OFF;
 #endif
 }
 
@@ -158,7 +192,7 @@ RN_DEVICE double rn_log_accept(double deltaH) {  // LeapFrog.scala:141-145
 // NVRTC time and megabytes of SASS for nothing -- the row loop dominates, not the call.
 __device__ __noinline__ void rn_update(const RnArgs& A, RnW& w, RnStats& S) {
   double dens;
-  rn_density(w.q, dens, w.g, w.scr, A.data, S.err, w.tma);
+  rn_density(w.q, dens, w.g, w.scr RN_DENSITY_RED(w.red), A.data, S.err, w.tma);
   w.U = dens * -1;
   S.grads += 1;
 }
@@ -272,7 +306,7 @@ RN_GLOBAL void rn_k_init(const RnArgs A) {
   const int c = (int)((blockIdx.x * blockDim.x + threadIdx.x) / RN_G);
   if (c >= A.chains) return;  // whole warp exits
   RnW w;
-  rn_w_setup(w, rn_smem + (size_t)RN_GROUP * RN_WPC_SMEM_DOUBLES);
+  rn_w_setup(w, rn_smem + (size_t)RN_GROUP * RN_WPC_SMEM_DOUBLES, RN_WPC_GSLICE(A.wpc_state, c));
   w.mass_kind = 0;
   RnRng rng;
   rng.seed = A.rng_seed[c];
@@ -368,7 +402,7 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
 #endif
   if (c >= A.chain_end) return;
   RnW w;
-  rn_w_setup(w, rn_smem + (size_t)RN_GROUP * RN_WPC_SMEM_DOUBLES);
+  rn_w_setup(w, rn_smem + (size_t)RN_GROUP * RN_WPC_SMEM_DOUBLES, RN_WPC_GSLICE(A.wpc_state, c));  // c: the absolute chain index
 #if RN_TMA_STAGES > 0
   if (lockstep) {
     const int first = A.chain_begin + (int)(blockIdx.x * (blockDim.x / RN_G));
@@ -588,7 +622,7 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
               RN_AT(A.est_mean, i, c) = 0.0;
               RN_AT(A.est_raw, i, c) = 0.0;
             }
-            S.err |= (int)rn_group_or((unsigned)(S.err & 2), w.scr + RN_WPC_RED_OFF);
+            S.err |= (int)rn_group_or((unsigned)(S.err & 2), w.red);
             RN_SYNC();
 #ifndef RN_HOST_EMULATION
             __threadfence_block();  // the matrix written lane-strided above is read by lane 0 below
@@ -653,7 +687,7 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
             RN_AT(A.est_raw, i, c) = raw;
           }
           if (window_end) {
-            S.err |= (int)rn_group_or((unsigned)(S.err & 2), w.scr + RN_WPC_RED_OFF);
+            S.err |= (int)rn_group_or((unsigned)(S.err & 2), w.red);
             win_i = 0;
             win_size = rn_d2i(win_size * A.win_expansion);
             w.mass_kind = 1;
@@ -693,16 +727,16 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
 
 // =============================================================================================================
 RN_GLOBAL void rn_k_density(const double* RN_RESTRICT qin, double* RN_RESTRICT out, const double* data, int* err,
-                            int chains) {
+                            int chains, double* wpc_state = nullptr) {  // (null: placement 0, or the host emulation)
   const int c = (int)((blockIdx.x * blockDim.x + threadIdx.x) / RN_G);
   if (c >= chains) return;
   RnW w;
-  rn_w_setup(w, rn_smem + (size_t)RN_GROUP * RN_WPC_SMEM_DOUBLES);
+  rn_w_setup(w, rn_smem + (size_t)RN_GROUP * RN_WPC_SMEM_DOUBLES, RN_WPC_GSLICE(wpc_state, c));
   RN_FOR_LANES(i) w.q[i] = qin[(size_t)i * chains + c];
   RN_SYNC();
   int e = 0;
   double dens;
-  rn_density(w.q, dens, w.g, w.scr, data, e, w.tma);
+  rn_density(w.q, dens, w.g, w.scr RN_DENSITY_RED(w.red), data, e, w.tma);
   RN_SYNC();
   if (RN_LANE == 0) out[c] = dens;
   RN_FOR_LANES(i) out[(size_t)(i + 1) * chains + c] = w.g[i];
