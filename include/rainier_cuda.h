@@ -266,6 +266,42 @@ int rn_sampler_set_comm(rn_sampler* s, rn_comm* comm);
 int rn_sampler_comm_stats(rn_sampler* s, int64_t* calls, double* total_us);
 void rn_sampler_destroy(rn_sampler* s);
 
+/* ---- checkpoints of a staged sampler (byte format: rainier_ckpt.h; DESIGN.md 3.6) --------------------------------- */
+/* Between API calls a chain's whole state is on the device: a checkpoint copies it out, and a restore in a fresh handle --
+ * another process, another device -- continues with the same bits as the uninterrupted run (any split of a run into
+ * rn_sampler_warmup / rn_sampler_run calls already gives the same bits, DESIGN.md 3.2).
+ * rn_sampler_save: at any API boundary after rn_sampler_create (before the first warmup call, mid-warmup, mid-sampling);
+ * synchronises the sampler's stream.  buf == NULL: only *needed.  A page-locked buf (rn_host_alloc / rn_host_register)
+ * is written by DMA, a pageable one through the pinned staging ring of rn_sample's drain.  Device staging is bounded
+ * (two buffers of at most 128 MB).
+ * rn_sampler_restore: a new sampler whose chains are the blobs' chains, concatenated in order, with kernels built as
+ * rn_sampler_create builds them for `cfg`.  RN_E_INVALID, naming the first differing item, when: a blob is truncated,
+ * corrupted (checksum) or of another version; the model (fingerprint of its RIR and data) or n differs; a semantic
+ * config field differs (sampler and its parameters, the tuners and their parameters, adaptation, step_adaptation,
+ * math_mode, gradient_mode, stats_window, and warmup_iterations while warmup is unfinished); the resolved kernel shape
+ * differs (the warp-per-chain placement may); several blobs disagree, or are concatenated where chains are not independent
+ * (pooled adaptation before the end of warmup).  iterations, launch_iterations and the device may differ.
+ * rn_checkpoint_info / rn_checkpoint_slice need no device.  A slice is chains [begin, end) as a blob of its own; refused
+ * where chains are not independent, as above. */
+/* (a struct tag only: the name is also the function's) */
+struct rn_checkpoint_info {
+  int32_t version;
+  int32_t phase;          /* 0 created, 1 warming up, 2 warmup finished, 3 sampling */
+  int64_t n, chains, chain_offset;
+  int32_t warmup_iterations, warm_done;
+  int32_t win_size, win_i, win_j, est_samples;
+  int32_t mass_kind, track;
+  int32_t track_thin, reserved;
+  int64_t track_seen, track_kept;
+  int32_t backend, wpc_k, mma, wpc_place; /* resolved shape: backend 0 thread per chain, 1 warp per chain */
+  uint64_t fingerprint;
+  uint64_t header_bytes, table_bytes, replicated_bytes, record_bytes, records_bytes, total_bytes;
+};
+int rn_sampler_save(rn_sampler* s, void* buf, size_t cap, size_t* needed);
+int rn_sampler_restore(rn_model* m, const rn_config* cfg, const void* const* blobs, const size_t* lens, int n_blobs, rn_sampler** out);
+int rn_checkpoint_info(const void* blob, size_t len, struct rn_checkpoint_info* out);
+int rn_checkpoint_slice(const void* blob, size_t len, int64_t begin, int64_t end, void* out, size_t cap, size_t* needed);
+
 /* ---- multi-GPU plumbing (one process per GPU; chains are sharded by the caller) ------------------------- */
 /* NCCL unique id exchange is the caller's job (e.g. torch.distributed broadcast of the 128 bytes). */
 int rn_comm_unique_id(char id[128]);

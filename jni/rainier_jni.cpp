@@ -281,6 +281,48 @@ JNIEXPORT void JNICALL Java_com_stripe_rainier_cuda_Native_samplerTrackedDiagnos
   if (rn_sampler_tracked_diagnostics((rn_sampler*)(intptr_t)s, vo.data()) != RN_OK) return throw_last(env);
   out_doubles(env, out, vo.data(), vo.size());
 }
+// ---- checkpoints of a staged sampler (rn_sampler_save / rn_sampler_restore); blobs travel in direct ByteBuffers ----
+// def samplerSave(sampler: Long, out: ByteBuffer /* direct, or null: size only */): Long   (bytes of the checkpoint)
+JNIEXPORT jlong JNICALL Java_com_stripe_rainier_cuda_Native_samplerSave(JNIEnv* env, jclass, jlong s, jobject out) {
+  size_t need = 0;
+  void* p = out ? env->GetDirectBufferAddress(out) : nullptr;
+  const size_t cap = out ? (size_t)env->GetDirectBufferCapacity(out) : 0;
+  if (rn_sampler_save((rn_sampler*)(intptr_t)s, p, cap, &need) != RN_OK) throw_last(env);
+  return (jlong)need;
+}
+// def samplerRestore(model: Long, config: ByteBuffer, blobs: Array[ByteBuffer], lens: Array[Long]): Long   (an rn_sampler handle)
+JNIEXPORT jlong JNICALL Java_com_stripe_rainier_cuda_Native_samplerRestore(JNIEnv* env, jclass, jlong m, jobject config, jobjectArray blobs,
+                                                                           jlongArray lens) {
+  const jsize k = env->GetArrayLength(blobs);
+  std::vector<const void*> ptrs((size_t)k);
+  for (jsize i = 0; i < k; i++) ptrs[i] = env->GetDirectBufferAddress(env->GetObjectArrayElement(blobs, i));
+  const std::vector<int64_t> l64 = in_longs(env, lens);
+  const std::vector<size_t> ls(l64.begin(), l64.end());
+  rn_sampler* s = nullptr;
+  if (rn_sampler_restore((rn_model*)(intptr_t)m, (const rn_config*)env->GetDirectBufferAddress(config), ptrs.data(), ls.data(), (int)k,
+                         &s) != RN_OK) {
+    throw_last(env);
+    return 0;
+  }
+  return (jlong)(intptr_t)s;
+}
+// def checkpointInfo(blob: ByteBuffer, len: Long, out: Array[Long]): Unit
+//   out = [version, phase, n, chains, chainOffset, warmDone, trackKept, totalBytes]
+JNIEXPORT void JNICALL Java_com_stripe_rainier_cuda_Native_checkpointInfo(JNIEnv* env, jclass, jobject blob, jlong len, jlongArray out) {
+  struct rn_checkpoint_info i;
+  if (rn_checkpoint_info(env->GetDirectBufferAddress(blob), (size_t)len, &i) != RN_OK) return throw_last(env);
+  const jlong v[8] = {i.version, i.phase, i.n, i.chains, i.chain_offset, i.warm_done, i.track_kept, (jlong)i.total_bytes};
+  env->SetLongArrayRegion(out, 0, 8, v);
+}
+// def checkpointSlice(blob: ByteBuffer, len: Long, begin: Long, end: Long, out: ByteBuffer /* or null: size only */): Long
+JNIEXPORT jlong JNICALL Java_com_stripe_rainier_cuda_Native_checkpointSlice(JNIEnv* env, jclass, jobject blob, jlong len, jlong begin,
+                                                                            jlong end, jobject out) {
+  size_t need = 0;
+  void* p = out ? env->GetDirectBufferAddress(out) : nullptr;
+  const size_t cap = out ? (size_t)env->GetDirectBufferCapacity(out) : 0;
+  if (rn_checkpoint_slice(env->GetDirectBufferAddress(blob), (size_t)len, begin, end, p, cap, &need) != RN_OK) throw_last(env);
+  return (jlong)need;
+}
 JNIEXPORT jstring JNICALL Java_com_stripe_rainier_cuda_Native_lastError(JNIEnv* env, jclass) {
   return env->NewStringUTF(rn_last_error());
 }

@@ -85,3 +85,44 @@ class ChainStats(C.Structure):
 class OptimizeConfig(C.Structure):
     _fields_ = [("struct_size", C.c_int32), ("history", C.c_int32), ("eps", C.c_double), ("max_evaluations", C.c_int32),
                 ("math_mode", C.c_int32), ("gradient_mode", C.c_int32), ("backend", C.c_int32)]
+
+
+class CheckpointInfo(C.Structure):  # struct rn_checkpoint_info
+    _fields_ = [("version", C.c_int32), ("phase", C.c_int32), ("n", C.c_int64), ("chains", C.c_int64), ("chain_offset", C.c_int64),
+                ("warmup_iterations", C.c_int32), ("warm_done", C.c_int32), ("win_size", C.c_int32), ("win_i", C.c_int32),
+                ("win_j", C.c_int32), ("est_samples", C.c_int32), ("mass_kind", C.c_int32), ("track", C.c_int32),
+                ("track_thin", C.c_int32), ("reserved", C.c_int32), ("track_seen", C.c_int64), ("track_kept", C.c_int64),
+                ("backend", C.c_int32), ("wpc_k", C.c_int32), ("mma", C.c_int32), ("wpc_place", C.c_int32),
+                ("fingerprint", C.c_uint64), ("header_bytes", C.c_uint64), ("table_bytes", C.c_uint64),
+                ("replicated_bytes", C.c_uint64), ("record_bytes", C.c_uint64), ("records_bytes", C.c_uint64),
+                ("total_bytes", C.c_uint64)]
+
+
+# the checkpoint byte format, include/rainier_ckpt.h
+CKPT_MAGIC = b"RNCKPT\0\1"
+CKPT_VERSION = 1
+(CKPT_PARAMS, CKPT_GRAD, CKPT_RNG_SEED, CKPT_RNG_NNG, CKPT_DA, CKPT_MASS, CKPT_CHOL, CKPT_EST_MEAN, CKPT_EST_RAW, CKPT_EST_COV, CKPT_RING,
+ CKPT_ST_GRADS, CKPT_ST_STEPS, CKPT_ST_ENERGY, CKPT_ST_RINGS, CKPT_TRACK, CKPT_RNG_HAVE, CKPT_DA_ITER, CKPT_RING_I, CKPT_RING_FULL,
+ CKPT_ST_ERR, CKPT_ST_ITERS, CKPT_ST_ACCEPTED, CKPT_ST_ENERGY_N, CKPT_ST_RING_I, CKPT_ST_RING_FULL) = range(1, 27)
+CKPT_F64, CKPT_I64, CKPT_I32 = 0, 1, 2
+
+
+class CkptField(C.Structure):  # rn_ckpt_field
+    _fields_ = [("id", C.c_uint32), ("type", C.c_uint32), ("elems", C.c_uint64)]
+
+
+class CkptHeader(C.Structure):  # rn_ckpt_header
+    _fields_ = [("magic", C.c_char * 8), ("version", C.c_uint32), ("header_bytes", C.c_uint32), ("fingerprint", C.c_uint64)] + \
+        [(f, C.c_int32) for f in ("sampler", "n_steps", "max_steps", "min_steps", "buf_size", "step_size_tuner", "step_adaptation",
+                                  "mass_tuner")] + \
+        [(f, C.c_double) for f in ("p_count", "delta", "static_step_size", "window_expansion")] + \
+        [(f, C.c_int32) for f in ("initial_window_size", "skip_first", "skip_last", "static_matrix", "adaptation", "math_mode",
+                                  "gradient_mode", "stats_window", "warmup_iterations", "iterations", "backend", "wpc_k", "mma",
+                                  "mma_chains", "wpc_place", "mass_max", "adjoint", "fast", "ehmc", "step_pool", "mass_pool",
+                                  "reserved0")] + \
+        [(f, C.c_int64) for f in ("n", "chains", "chain_offset")] + \
+        [(f, C.c_int32) for f in ("initialized", "warm_done", "stats_reset_for_sampling", "win_size", "win_i", "win_j", "est_samples",
+                                  "mass_kind", "track", "track_thin")] + \
+        [("track_seen", C.c_int64), ("track_kept", C.c_int64), ("sampling_ms", C.c_double), ("track_ms", C.c_double),
+         ("sampling_iterations", C.c_int64), ("n_fields", C.c_uint32), ("reserved1", C.c_uint32), ("step_bytes", C.c_uint64),
+         ("pool_bytes", C.c_uint64), ("record_bytes", C.c_uint64)]

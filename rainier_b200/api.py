@@ -125,6 +125,11 @@ def lib():
         L.rn_generator_destroy.argtypes = [C.c_void_p]
         L.rn_sample_generate.argtypes = [C.c_void_p, C.POINTER(Config), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                          C.c_void_p]
+        L.rn_sampler_save.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.rn_sampler_restore.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int,
+                                         C.POINTER(C.c_void_p)]
+        L.rn_checkpoint_info.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(abi.CheckpointInfo)]
+        L.rn_checkpoint_slice.argtypes = [C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
         sizes = (C.c_int32 * 4)()
         L.rn_abi_sizes(sizes)
         if sizes[0] != C.sizeof(Config) or sizes[1] != C.sizeof(ChainStats) or sizes[2] != C.sizeof(RngState):
@@ -830,6 +835,33 @@ class Comm:
             self.h = None
 
 
+def _blob_view(blob):
+    """a bytes-like checkpoint (bytes, bytearray, memoryview, numpy array) as a flat uint8 array over the same memory"""
+    a = blob if isinstance(blob, np.ndarray) else np.frombuffer(blob, dtype=np.uint8)
+    if not a.flags.c_contiguous:
+        raise ValueError("a checkpoint must be one contiguous buffer")
+    return a.reshape(-1).view(np.uint8)
+
+
+def checkpoint_info(blob):
+    """rn_checkpoint_info: what a sampler checkpoint holds (no device needed), as a dict"""
+    a = _blob_view(blob)
+    info = abi.CheckpointInfo()
+    _check(lib().rn_checkpoint_info(a.ctypes.data, a.nbytes, C.byref(info)))
+    return {f: getattr(info, f) for f, _ in abi.CheckpointInfo._fields_ if f != "reserved"}
+
+
+def checkpoint_slice(blob, begin, end):
+    """rn_checkpoint_slice: chains [begin, end) of a checkpoint as a checkpoint of their own (bytearray; no device needed)"""
+    a = _blob_view(blob)
+    need = C.c_size_t(0)
+    _check(lib().rn_checkpoint_slice(a.ctypes.data, a.nbytes, int(begin), int(end), None, 0, C.byref(need)))
+    out = bytearray(need.value)
+    _check(lib().rn_checkpoint_slice(a.ctypes.data, a.nbytes, int(begin), int(end), (C.c_char * len(out)).from_buffer(out), len(out),
+                                     C.byref(need)))
+    return out
+
+
 class CudaSampler:
     """Staged, device-resident sampling (what rn_sample is built from); used by bench.py and the parity tests."""
 
@@ -913,6 +945,43 @@ class CudaSampler:
         rings = np.zeros((self.chains, 3, self.cfg.stats_window), dtype=np.float64)
         _check(lib().rn_sampler_stats(self.h, C.cast(stats, C.c_void_p), mass.ctypes.data, rings.ctypes.data))
         return [Stats(stats[c], rings[c]) for c in range(self.chains)], mass
+
+    def save(self, out=None):
+        """rn_sampler_save: the sampler's whole state as a checkpoint (DESIGN.md 3.6).  Returns a bytearray, or, with `out` (a
+        uint8 numpy array of at least the size, e.g. PinnedBuffer(..., dtype=np.uint8).array: one DMA per chunk), the view of
+        `out` that holds it."""
+        need = C.c_size_t(0)
+        _check(lib().rn_sampler_save(self.h, None, 0, C.byref(need)))
+        if out is None:
+            buf = bytearray(need.value)
+            _check(lib().rn_sampler_save(self.h, (C.c_char * len(buf)).from_buffer(buf), len(buf), C.byref(need)))
+            return buf
+        a = _blob_view(out)
+        if a.nbytes < need.value:
+            raise ValueError("out holds %d bytes, the checkpoint needs %d" % (a.nbytes, need.value))
+        _check(lib().rn_sampler_save(self.h, a.ctypes.data, a.nbytes, C.byref(need)))
+        return a[:need.value]
+
+    @classmethod
+    def restore(cls, model, config, blobs, trace=False):
+        """rn_sampler_restore: a new sampler whose chains are those of `blobs` (one checkpoint or a list), concatenated in
+        order, continuing exactly where they were saved.  `config` must agree with the checkpoints' semantic fields; its
+        iterations may be larger (extension).  trace=True records the per-iteration trace from the restore point on."""
+        views = [_blob_view(b) for b in (blobs if isinstance(blobs, (list, tuple)) else [blobs])]
+        self = cls.__new__(cls)
+        self.model = model
+        self.cfg, self._keep = lower_config(config)
+        ptrs = (C.c_void_p * len(views))(*[v.ctypes.data for v in views])
+        lens = (C.c_size_t * len(views))(*[v.nbytes for v in views])
+        h = C.c_void_p()
+        _check(lib().rn_sampler_restore(model.h, C.byref(self.cfg), ptrs, lens, len(views), C.byref(h)))
+        self.h = h
+        self.chains = sum(checkpoint_info(v)["chains"] for v in views)
+        self.cfg.warmup_iterations = checkpoint_info(views[0])["warmup_iterations"]  # (may differ only once warmup has finished)
+        self._trace = trace
+        if trace:
+            _check(lib().rn_sampler_enable_trace(self.h))
+        return self
 
     def read_trace(self):
         total = self.cfg.warmup_iterations + self.cfg.iterations

@@ -267,6 +267,9 @@ struct rn_model {
     long long global_doubles = 0;  // backend 1: per-start slice of the global state array (RnOptArgs::wpc_state)
   };
   std::map<std::tuple<bool, bool, int, int>, std::unique_ptr<OptKernel>> opt_kernels;
+  // checkpoints: hash of the RIR bytes and the device data image, computed on the first save or restore (rn_ckpt_header)
+  bool has_fingerprint = false;
+  uint64_t fingerprint = 0;
 };
 
 static int make_current(const Api* A, rn_model* m) {
@@ -1123,6 +1126,7 @@ struct rn_sampler {
   size_t track_draws_bytes = 0;
   std::vector<std::pair<CUevent, CUevent>> track_events;  // not yet folded into track_ms
   double track_ms = 0.0;
+  int64_t chain_offset = 0;  // a restored sampler: index of its first chain in the sampler that was saved (rn_ckpt_header)
 };
 
 namespace {
@@ -1944,6 +1948,18 @@ int rn_sampler_diagnostics(rn_sampler* s, const double* d_samples, int iteration
   return RN_OK;
 }
 
+// the tracker's device buffers (state, finish scratch), allocated once per sampler; also by rn_sampler_restore
+static int track_alloc(const Api* A, rn_sampler* s) {
+  const size_t n = s->m->n_params, nC = n * (size_t)s->chains, bytes = (size_t)RN_DIAG_STATE_DOUBLES * nC * 8;
+  if (!s->d_track) {  // the finish allocates nothing, so a rank cannot fail there on memory while the others all-reduce
+    CU(A->cuMemAlloc(&s->d_track, std::max<size_t>(bytes, 8)));
+    CU(A->cuMemAlloc(&s->d_track_terms, (size_t)kTermRows * nC * 8));
+    CU(A->cuMemAlloc(&s->d_track_sums, (5 + n + (2 + (size_t)RN_DIAG_LAGS) * n + n) * 8));
+    CU(A->cuFuncSetAttribute(s->K->k_diag_accum, 8 /*MAX_DYNAMIC_SHARED_SIZE_BYTES*/, (99 + kTrackSub) * kTrackThreads * 8));
+  }
+  return RN_OK;
+}
+
 // Trace.thin(thin).diagnostics from here on, accumulated after every sampling launch (track_accumulate, rn_k_diag_accum)
 int rn_sampler_track_diagnostics(rn_sampler* s, int thin) {
   if (!s) return fail(RN_E_INVALID, "null sampler");
@@ -1953,13 +1969,9 @@ int rn_sampler_track_diagnostics(rn_sampler* s, int thin) {
   const Api* A = api(&why);
   if (!A) return fail(RN_E_CUDA, why);
   CU(A->cuCtxSetCurrent(s->m->ctx));
-  const size_t n = s->m->n_params, nC = n * (size_t)s->chains, bytes = (size_t)RN_DIAG_STATE_DOUBLES * nC * 8;
-  if (!s->d_track) {  // the finish allocates nothing, so a rank cannot fail there on memory while the others all-reduce
-    CU(A->cuMemAlloc(&s->d_track, std::max<size_t>(bytes, 8)));
-    CU(A->cuMemAlloc(&s->d_track_terms, (size_t)kTermRows * nC * 8));
-    CU(A->cuMemAlloc(&s->d_track_sums, (5 + n + (2 + (size_t)RN_DIAG_LAGS) * n + n) * 8));
-    CU(A->cuFuncSetAttribute(s->K->k_diag_accum, 8 /*MAX_DYNAMIC_SHARED_SIZE_BYTES*/, (99 + kTrackSub) * kTrackThreads * 8));
-  }
+  const size_t bytes = (size_t)RN_DIAG_STATE_DOUBLES * s->m->n_params * (size_t)s->chains * 8;
+  int rc = track_alloc(A, s);
+  if (rc) return rc;
   CU(A->cuMemsetD8Async(s->d_track, 0, bytes, s->stream));
   s->track = true;
   s->track_thin = thin;
@@ -3551,6 +3563,613 @@ int rn_sample_generate(rn_model* m, const rn_config* cfg, rn_generator* g, const
     if (rc) return rc;
   }
   if (stats) std::memcpy(stats, st.data(), C * sizeof(rn_chain_stats));
+  return RN_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------
+// checkpoints of a staged sampler (rn_sampler_save / rn_sampler_restore; byte format: rainier_ckpt.h; DESIGN.md 3.6).
+// At an API boundary a chain's whole state is the SoA arena plus the tracked-diagnostics state and a few host-mirrored
+// counters: the warp-per-chain slices of placement 1 and the thread shape's on-chip restore point hold nothing between
+// launches.  rn_state.cuh transposes the arena to chain-major records and back, in a module of its own (state_module), in
+// chunks of chains through a bounded device staging buffer.
+// ---------------------------------------------------------------------------------------------------------
+#include "../../include/rainier_ckpt.h"
+#define RN_STATE_ARGS_ONLY
+#include "rn_state.cuh"
+#undef RN_STATE_ARGS_ONLY
+
+namespace rn {
+extern const char* kStateSource;  // rn_state.cuh, embedded at build time
+}
+
+static_assert(sizeof(rn_ckpt_header) == 312 && sizeof(rn_ckpt_field) == 16, "rainier_ckpt.h: no implicit padding");
+static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "checkpoints are little-endian byte images");
+
+namespace {
+
+const uint64_t kFnvBasis = 1469598103934665603ull, kFnvPrime = 1099511628211ull;
+
+// four interleaved FNV-1a-style lanes over 64-bit words: every step is a bijection of the lane, so a changed word always
+// changes the result
+uint64_t hash_words(const uint8_t* p, size_t len) {
+  uint64_t h[4] = {kFnvBasis, kFnvBasis ^ 1, kFnvBasis ^ 2, kFnvBasis ^ 3};
+  const size_t words = len / 8;
+  size_t i = 0;
+  for (; i + 4 <= words; i += 4)
+    for (int l = 0; l < 4; l++) {
+      uint64_t w;
+      std::memcpy(&w, p + (i + l) * 8, 8);
+      h[l] = (h[l] ^ w) * kFnvPrime;
+    }
+  for (; i < words; i++) {
+    uint64_t w;
+    std::memcpy(&w, p + i * 8, 8);
+    h[i & 3] = (h[i & 3] ^ w) * kFnvPrime;
+  }
+  uint64_t tail = 0;
+  std::memcpy(&tail, p + words * 8, len - words * 8);
+  uint64_t r = (kFnvBasis ^ tail) * kFnvPrime;
+  for (int l = 0; l < 4; l++) r = (r ^ h[l]) * kFnvPrime;
+  return (r ^ (uint64_t)len) * kFnvPrime;
+}
+
+// the checksum of a blob: hash_words of 16 MB segments (on up to 16 threads), then of the segments' hashes
+uint64_t blob_hash(const uint8_t* p, size_t len) {
+  const size_t seg = (size_t)16 << 20, nseg = std::max<size_t>(1, (len + seg - 1) / seg);
+  std::vector<uint64_t> hs(nseg);
+  auto work = [&](size_t k) { hs[k] = hash_words(p + k * seg, std::min(seg, len - std::min(len, k * seg))); };
+  const size_t T = std::min<size_t>(nseg, std::max(1u, std::min(16u, std::thread::hardware_concurrency())));
+  if (T <= 1) {
+    for (size_t k = 0; k < nseg; k++) work(k);
+  } else {
+    std::atomic<size_t> next{0};
+    std::vector<std::thread> th;
+    for (size_t t = 0; t < T; t++)
+      th.emplace_back([&] {
+        for (size_t k; (k = next.fetch_add(1)) < nseg;) work(k);
+      });
+    for (auto& t : th) t.join();
+  }
+  return hash_words((const uint8_t*)hs.data(), hs.size() * 8);
+}
+
+// the model's fingerprint: its RIR bytes and the data image on the device (computed once)
+int model_fingerprint(const Api* A, rn_model* m, uint64_t* out) {
+  if (!m->has_fingerprint) {
+    std::vector<uint8_t> img((size_t)m->data_doubles * 8);
+    if (!img.empty()) CU(A->cuMemcpyDtoH(img.data(), m->d_data, img.size()));
+    const uint64_t parts[3] = {blob_hash(m->rir.data(), m->rir.size()), blob_hash(img.data(), img.size()), (uint64_t)m->n_params};
+    m->fingerprint = hash_words((const uint8_t*)parts, sizeof(parts));
+    m->has_fingerprint = true;
+  }
+  *out = m->fingerprint;
+  return RN_OK;
+}
+
+struct StateModule {
+  CUmodule mod = nullptr;
+  CUfunction pack = nullptr, unpack = nullptr;
+};
+// rn_state.cuh compiled once per process and loaded once per device (in its primary context, which host_ctx keeps alive)
+int state_module(const Api* A, int device, const StateModule** out) {
+  static std::mutex mu;
+  static std::vector<char> cubin;
+  static std::map<int, StateModule> mods;
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = mods.find(device);
+  if (it == mods.end()) {
+    if (cubin.empty()) {
+      const int rc = nvrtc_to_cubin(kStateSource, "rainier_state.cu", false, cubin);
+      if (rc) return rc;
+    }
+    StateModule M;
+    CU(A->cuModuleLoadData(&M.mod, cubin.data()));
+    CU(A->cuModuleGetFunction(&M.pack, M.mod, "rn_k_state_pack"));
+    CU(A->cuModuleGetFunction(&M.unpack, M.mod, "rn_k_state_unpack"));
+    it = mods.emplace(device, M).first;
+  }
+  *out = &it->second;
+  return RN_OK;
+}
+
+struct CkptField {
+  rn_ckpt_field f;
+  CUdeviceptr ptr;
+};
+uint64_t ckpt_type_bytes(uint32_t type) { return type == RN_CKPT_I32 ? 4 : 8; }
+
+// the record layout of a sampler's state: 8-byte fields, then 4-byte ones, each with its device array (empty fields omitted)
+std::vector<CkptField> ckpt_layout(const rn_sampler* s, uint64_t* record_bytes) {
+  const RnArgs& a = s->args;
+  const uint64_t n = s->m->n_params, W = (uint64_t)s->cfg.stats_window;
+  const int mass_max = key_for(s->m, &s->cfg).mass_max;
+  const bool dense = mass_max == 2, diag = mass_max >= 1, ehmc = s->cfg.sampler == RN_SAMPLER_EHMC;
+  std::vector<CkptField> L;
+  auto add = [&](uint32_t id, uint32_t type, uint64_t elems, const void* p) {
+    if (elems) L.push_back({{id, type, elems}, (CUdeviceptr)(uintptr_t)p});
+  };
+  add(RN_CKPT_PARAMS, RN_CKPT_F64, 2 * n + 1, a.params);
+  add(RN_CKPT_GRAD, RN_CKPT_F64, n, a.grad);
+  add(RN_CKPT_RNG_SEED, RN_CKPT_I64, 1, a.rng_seed);
+  add(RN_CKPT_RNG_NNG, RN_CKPT_F64, 1, a.rng_nng);
+  add(RN_CKPT_DA, RN_CKPT_F64, 5, a.da);
+  add(RN_CKPT_MASS, RN_CKPT_F64, dense ? n * n : (diag ? n : 0), a.mass);
+  add(RN_CKPT_CHOL, RN_CKPT_F64, dense ? n * (n + 1) / 2 : 0, a.chol);
+  add(RN_CKPT_EST_MEAN, RN_CKPT_F64, diag ? n : 0, a.est_mean);
+  add(RN_CKPT_EST_RAW, RN_CKPT_F64, diag ? n : 0, a.est_raw);
+  add(RN_CKPT_EST_COV, RN_CKPT_F64, dense ? n * n : 0, a.est_cov);
+  add(RN_CKPT_RING, RN_CKPT_F64, ehmc ? (uint64_t)s->cfg.buf_size : 0, a.ring);
+  add(RN_CKPT_ST_GRADS, RN_CKPT_I64, 1, a.st_grads);
+  add(RN_CKPT_ST_STEPS, RN_CKPT_I64, 1, a.st_steps);
+  add(RN_CKPT_ST_ENERGY, RN_CKPT_F64, 3, a.st_energy);
+  add(RN_CKPT_ST_RINGS, RN_CKPT_F64, 3 * W, a.st_rings);
+  add(RN_CKPT_TRACK, RN_CKPT_F64, s->track ? (uint64_t)RN_DIAG_STATE_DOUBLES * n : 0, (const void*)(uintptr_t)s->d_track);
+  add(RN_CKPT_RNG_HAVE, RN_CKPT_I32, 1, a.rng_have);
+  add(RN_CKPT_DA_ITER, RN_CKPT_I32, 1, a.da_iter);
+  add(RN_CKPT_RING_I, RN_CKPT_I32, 1, a.ring_i);
+  add(RN_CKPT_RING_FULL, RN_CKPT_I32, 1, a.ring_full);
+  add(RN_CKPT_ST_ERR, RN_CKPT_I32, 1, a.st_err);
+  add(RN_CKPT_ST_ITERS, RN_CKPT_I32, 1, a.st_iters);
+  add(RN_CKPT_ST_ACCEPTED, RN_CKPT_I32, 1, a.st_accepted);
+  add(RN_CKPT_ST_ENERGY_N, RN_CKPT_I32, 1, a.st_energy_n);
+  add(RN_CKPT_ST_RING_I, RN_CKPT_I32, 3, a.st_ring_i);
+  add(RN_CKPT_ST_RING_FULL, RN_CKPT_I32, 3, a.st_ring_full);
+  uint64_t bytes = 0;
+  for (const CkptField& F : L) bytes += F.f.elems * ckpt_type_bytes(F.f.type);
+  *record_bytes = (bytes + 7) & ~(uint64_t)7;
+  return L;
+}
+
+uint64_t ckpt_step_bytes(const rn_config& c) {  // rn_sampler_create's d_step
+  return c.step_adaptation == RN_ADAPT_POOLED ? (2 + (uint64_t)c.warmup_iterations) * 8 : 8;
+}
+
+void ckpt_header(const rn_sampler* s, const std::vector<CkptField>& L, uint64_t record_bytes, rn_ckpt_header& h) {
+  std::memset(&h, 0, sizeof(h));
+  std::memcpy(h.magic, RN_CKPT_MAGIC, 8);
+  h.version = RN_CKPT_VERSION;
+  h.header_bytes = (uint32_t)sizeof(h);
+  const rn_config& c = s->cfg;
+  h.sampler = c.sampler, h.n_steps = c.n_steps, h.max_steps = c.max_steps, h.min_steps = c.min_steps, h.buf_size = c.buf_size;
+  h.step_size_tuner = c.step_size_tuner, h.step_adaptation = c.step_adaptation, h.mass_tuner = c.mass_tuner;
+  h.p_count = c.p_count, h.delta = c.delta, h.static_step_size = c.static_step_size, h.window_expansion = c.window_expansion;
+  h.initial_window_size = c.initial_window_size, h.skip_first = c.skip_first, h.skip_last = c.skip_last;
+  h.static_matrix = c.static_matrix, h.adaptation = c.adaptation, h.math_mode = c.math_mode, h.gradient_mode = c.gradient_mode;
+  h.stats_window = c.stats_window, h.warmup_iterations = c.warmup_iterations, h.iterations = c.iterations;
+  const Kernel& K = *s->K;
+  const KernelKey key = key_for(s->m, &c);
+  h.backend = K.backend, h.wpc_k = K.backend ? K.wpc_k : 0, h.mma = K.mma ? 1 : 0, h.mma_chains = K.mma ? K.mma_chains : 0;
+  h.wpc_place = K.backend ? K.wpc_place : 0, h.mass_max = key.mass_max, h.adjoint = key.adjoint;
+  h.fast = key.fast, h.ehmc = key.ehmc, h.step_pool = K.step_pool, h.mass_pool = K.mass_pool;
+  h.n = s->m->n_params, h.chains = s->chains, h.chain_offset = s->chain_offset;
+  h.initialized = s->initialized, h.warm_done = s->warm_done, h.stats_reset_for_sampling = s->stats_reset_for_sampling;
+  h.win_size = s->win_size, h.win_i = s->win_i, h.win_j = s->win_j, h.est_samples = s->est_samples, h.mass_kind = s->mass_kind;
+  h.track = s->track, h.track_thin = s->track_thin, h.track_seen = s->track_seen, h.track_kept = s->track_kept;
+  h.sampling_ms = s->sampling_ms, h.track_ms = s->track_ms, h.sampling_iterations = s->sampling_iterations;
+  h.n_fields = (uint32_t)L.size();
+  h.step_bytes = ckpt_step_bytes(c);
+  h.pool_bytes = pool_doubles(s) * 8;
+  h.record_bytes = record_bytes;
+}
+
+struct CkptView {  // a parsed, verified blob
+  rn_ckpt_header h;
+  std::vector<rn_ckpt_field> table;
+  const uint8_t* p = nullptr;
+  uint64_t table_off = 0, rep_off = 0, rec_off = 0, total = 0;
+};
+
+std::string num(double v) {
+  std::ostringstream os;
+  os.precision(17);
+  os << v;
+  return os.str();
+}
+
+int ckpt_parse(const void* blob, size_t len, const std::string& what, CkptView* v) {
+  if (!blob) return fail(RN_E_INVALID, what + ": null blob");
+  if (len < sizeof(rn_ckpt_header))
+    return fail(RN_E_INVALID, what + ": truncated (" + std::to_string(len) + " bytes, shorter than the header)");
+  rn_ckpt_header& h = v->h;
+  std::memcpy(&h, blob, sizeof(h));
+  if (std::memcmp(h.magic, RN_CKPT_MAGIC, 8) != 0) return fail(RN_E_INVALID, what + ": not a sampler checkpoint (bad magic)");
+  if (h.version != RN_CKPT_VERSION)
+    return fail(RN_E_INVALID, what + ": version " + std::to_string(h.version) + ", this library reads version " +
+                                  std::to_string(RN_CKPT_VERSION));
+  if (h.header_bytes != sizeof(h) || h.n_fields > RN_STATE_MAX_FIELDS || h.chains < 1 || h.chains > INT32_MAX || h.n < 1 ||
+      h.record_bytes % 8 != 0 || h.record_bytes > ((uint64_t)1 << 40) || h.step_bytes > ((uint64_t)1 << 40) ||
+      h.pool_bytes > ((uint64_t)1 << 40))
+    return fail(RN_E_INVALID, what + ": malformed header");
+  v->p = (const uint8_t*)blob;
+  v->table_off = sizeof(h);
+  v->rep_off = v->table_off + (uint64_t)h.n_fields * sizeof(rn_ckpt_field);
+  v->rec_off = v->rep_off + h.step_bytes + h.pool_bytes;
+  const uint64_t records = (uint64_t)h.chains * h.record_bytes;
+  if (h.record_bytes && records / h.record_bytes != (uint64_t)h.chains) return fail(RN_E_INVALID, what + ": malformed header");
+  v->total = v->rec_off + records + 8;
+  if (len < v->total)
+    return fail(RN_E_INVALID, what + ": truncated (" + std::to_string(len) + " of " + std::to_string(v->total) + " bytes)");
+  if (len > v->total) return fail(RN_E_INVALID, what + ": " + std::to_string(len - v->total) + " bytes after the checksum");
+  uint64_t sum;
+  std::memcpy(&sum, v->p + v->total - 8, 8);
+  if (sum != blob_hash(v->p, v->total - 8)) return fail(RN_E_INVALID, what + ": checksum mismatch (corrupted blob)");
+  v->table.resize(h.n_fields);
+  std::memcpy(v->table.data(), v->p + v->table_off, v->table.size() * sizeof(rn_ckpt_field));
+  uint64_t bytes = 0;
+  for (const rn_ckpt_field& f : v->table) {
+    if (f.type > RN_CKPT_I32 || f.elems > ((uint64_t)1 << 36)) return fail(RN_E_INVALID, what + ": malformed field table");
+    bytes += f.elems * ckpt_type_bytes(f.type);
+  }
+  if (((bytes + 7) & ~(uint64_t)7) != h.record_bytes) return fail(RN_E_INVALID, what + ": field table does not match the record size");
+  return RN_OK;
+}
+
+// chains of a blob are independent -- may be cut apart or joined with other blobs' -- unless a pooled adaptation is still
+// warming up: pooled windows sum per rank, then over ranks, so their bits depend on how the chains are split (DESIGN.md 5)
+bool ckpt_independent(const rn_ckpt_header& h) {
+  const bool pooled = h.adaptation == RN_ADAPT_POOLED || h.step_adaptation == RN_ADAPT_POOLED;
+  return !pooled || (h.initialized && h.warm_done == h.warmup_iterations);
+}
+
+// two blobs that are to be restored as one sampler: everything but the chain count, the offset and the device times agrees
+int ckpt_same(const CkptView& a, const CkptView& b, const std::string& what) {
+#define RN_CKPT_SAME(f) \
+  if (a.h.f != b.h.f) return fail(RN_E_INVALID, what + ": " #f " differs from the first checkpoint's (" + num((double)b.h.f) + " vs " + num((double)a.h.f) + ")");
+  RN_CKPT_SAME(fingerprint) RN_CKPT_SAME(n) RN_CKPT_SAME(sampler) RN_CKPT_SAME(n_steps) RN_CKPT_SAME(max_steps)
+  RN_CKPT_SAME(min_steps) RN_CKPT_SAME(buf_size) RN_CKPT_SAME(p_count) RN_CKPT_SAME(step_size_tuner) RN_CKPT_SAME(step_adaptation)
+  RN_CKPT_SAME(delta) RN_CKPT_SAME(static_step_size) RN_CKPT_SAME(mass_tuner) RN_CKPT_SAME(initial_window_size)
+  RN_CKPT_SAME(window_expansion) RN_CKPT_SAME(skip_first) RN_CKPT_SAME(skip_last) RN_CKPT_SAME(static_matrix)
+  RN_CKPT_SAME(adaptation) RN_CKPT_SAME(math_mode) RN_CKPT_SAME(gradient_mode) RN_CKPT_SAME(stats_window)
+  RN_CKPT_SAME(warmup_iterations) RN_CKPT_SAME(backend) RN_CKPT_SAME(wpc_k) RN_CKPT_SAME(mma) RN_CKPT_SAME(mma_chains)
+  RN_CKPT_SAME(mass_max) RN_CKPT_SAME(adjoint) RN_CKPT_SAME(fast) RN_CKPT_SAME(ehmc) RN_CKPT_SAME(step_pool) RN_CKPT_SAME(mass_pool)
+  RN_CKPT_SAME(initialized) RN_CKPT_SAME(warm_done) RN_CKPT_SAME(stats_reset_for_sampling) RN_CKPT_SAME(win_size)
+  RN_CKPT_SAME(win_i) RN_CKPT_SAME(win_j) RN_CKPT_SAME(est_samples) RN_CKPT_SAME(mass_kind) RN_CKPT_SAME(track)
+  RN_CKPT_SAME(track_thin) RN_CKPT_SAME(track_seen) RN_CKPT_SAME(track_kept) RN_CKPT_SAME(step_bytes) RN_CKPT_SAME(pool_bytes)
+  RN_CKPT_SAME(record_bytes)
+#undef RN_CKPT_SAME
+  if (a.table.size() != b.table.size() || std::memcmp(a.table.data(), b.table.data(), a.table.size() * sizeof(rn_ckpt_field)) != 0)
+    return fail(RN_E_INVALID, what + ": field table differs from the first checkpoint's");
+  return RN_OK;
+}
+
+// the semantic fields of the config a sampler is restored with must be the checkpoint's (warmup_iterations only while warmup
+// is unfinished: a finished run may be extended)
+int ckpt_config_matches(const rn_ckpt_header& h, const rn_config& c) {
+#define RN_CKPT_CFG(f) \
+  if ((double)h.f != (double)c.f) return fail(RN_E_INVALID, "rn_sampler_restore: rn_config." #f " differs (checkpoint " + num((double)h.f) + ", config " + num((double)c.f) + ")");
+  RN_CKPT_CFG(sampler) RN_CKPT_CFG(n_steps) RN_CKPT_CFG(max_steps) RN_CKPT_CFG(min_steps) RN_CKPT_CFG(buf_size) RN_CKPT_CFG(p_count)
+  RN_CKPT_CFG(step_size_tuner) RN_CKPT_CFG(step_adaptation) RN_CKPT_CFG(delta) RN_CKPT_CFG(static_step_size) RN_CKPT_CFG(mass_tuner)
+  RN_CKPT_CFG(initial_window_size) RN_CKPT_CFG(window_expansion) RN_CKPT_CFG(skip_first) RN_CKPT_CFG(skip_last)
+  RN_CKPT_CFG(static_matrix) RN_CKPT_CFG(adaptation) RN_CKPT_CFG(math_mode) RN_CKPT_CFG(gradient_mode) RN_CKPT_CFG(stats_window)
+  if (!(h.initialized && h.warm_done == h.warmup_iterations)) {
+    RN_CKPT_CFG(warmup_iterations)
+  }
+#undef RN_CKPT_CFG
+  return RN_OK;
+}
+
+// DMMA path: the whole groups of mma_chains chains take it, a ragged tail the per-warp path of the same kernel, so a chain must
+// keep its place relative to the groups
+bool ckpt_mma_aligned(const rn_ckpt_header& h, int64_t begin, int64_t end) {
+  if (!h.mma || h.mma_chains <= 0) return true;
+  return begin % h.mma_chains == 0 && (end == h.chains || (end - begin) % h.mma_chains == 0);
+}
+
+size_t ckpt_stage_bytes() {  // one of the two device staging buffers
+  size_t b = (size_t)128 << 20;
+  if (const char* e = getenv("RN_CKPT_STAGE")) b = std::max<size_t>(8, (size_t)atoll(e));
+  return b;
+}
+
+RnStateArgs ckpt_args(const rn_sampler* s, const std::vector<CkptField>& L, uint64_t record_bytes) {
+  RnStateArgs a;
+  std::memset(&a, 0, sizeof(a));
+  uint64_t off = 0;
+  for (size_t f = 0; f < L.size(); f++) {
+    const uint64_t tb = ckpt_type_bytes(L[f].f.type);
+    a.f[f].ptr = L[f].ptr;
+    a.f[f].elems = (long long)L[f].f.elems;
+    a.f[f].words = (int)(tb / 4);
+    a.f[f].rec_word = (int)(off / 4);
+    off += L[f].f.elems * tb;
+  }
+  a.n_fields = (int)L.size();
+  a.rec_words = (long long)(record_bytes / 4);
+  a.C = s->chains;
+  return a;
+}
+
+int state_launch(const Api* A, CUfunction f, RnStateArgs& a, CUstream st) {
+  const unsigned gx = (unsigned)((a.count + 31) / 32);
+  const unsigned gy = (unsigned)std::min<long long>(65535, std::max<long long>(1, (a.rec_words + 31) / 32));
+  void* params[] = {&a};
+  CU(A->cuLaunchKernel(f, gx, gy, 1, 32, RN_STATE_ROWS, 1, 0, st, params, nullptr));
+  return RN_OK;
+}
+
+// the device buffers and copy stream of one save or restore
+struct CkptStaging {
+  const Api* A;
+  CUdeviceptr buf[2] = {0, 0};
+  CUstream cs = nullptr;
+  CUevent ev[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // [buffer][0 filled on its producer, 1 drained by its consumer]
+  bool used[2] = {false, false};
+  ~CkptStaging() {
+    if (cs) A->cuStreamSynchronize(cs);
+    for (auto& p : ev)
+      for (CUevent e : p)
+        if (e) A->cuEventDestroy(e);
+    if (cs) A->cuStreamDestroy(cs);
+    for (CUdeviceptr b : buf)
+      if (b) A->cuMemFree(b);
+  }
+  int init(uint64_t bytes, int nbuf) {
+    CU(A->cuStreamCreate(&cs, 1 /*CU_STREAM_NON_BLOCKING*/));
+    for (int b = 0; b < nbuf; b++) {
+      CU(A->cuMemAlloc(&buf[b], bytes));
+      CU(A->cuEventCreate(&ev[b][0], 2 /*CU_EVENT_DISABLE_TIMING*/));
+      CU(A->cuEventCreate(&ev[b][1], 2));
+    }
+    return RN_OK;
+  }
+};
+
+// chains [0, C) -> records at dst: rn_k_state_pack of chunk k + 1 on the sampler's stream overlaps the copy of chunk k
+// (drain_to_host on the copy stream: one DMA into page-locked memory, else the pinned staging ring)
+int ckpt_save_records(const Api* A, rn_sampler* s, const std::vector<CkptField>& L, uint64_t R, uint8_t* dst) {
+  const StateModule* M = nullptr;
+  int rc = state_module(A, s->m->device, &M);
+  if (rc) return rc;
+  const int64_t C = s->chains, per = (int64_t)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)C, ckpt_stage_bytes() / R));
+  const int64_t chunks = (C + per - 1) / per;
+  CkptStaging S{A};
+  rc = S.init((uint64_t)per * R, chunks > 1 ? 2 : 1);
+  if (rc) return rc;
+  RnStateArgs a = ckpt_args(s, L, R);
+  auto pack = [&](int64_t k) -> int {
+    const int b = (int)(k & 1);
+    if (S.used[b]) CU(A->cuStreamWaitEvent(s->stream, S.ev[b][1], 0));
+    a.c0 = (long long)(k * per);
+    a.count = (long long)std::min<int64_t>(per, C - (int64_t)a.c0);
+    a.staging = (unsigned*)(uintptr_t)S.buf[b];
+    int r = state_launch(A, M->pack, a, s->stream);
+    if (r) return r;
+    CU(A->cuEventRecord(S.ev[b][0], s->stream));
+    S.used[b] = true;
+    return RN_OK;
+  };
+  rc = pack(0);
+  if (rc) return rc;
+  for (int64_t k = 0; k < chunks; k++) {
+    const int b = (int)(k & 1);
+    if (k + 1 < chunks) {
+      rc = pack(k + 1);
+      if (rc) return rc;
+    }
+    CU(A->cuStreamWaitEvent(S.cs, S.ev[b][0], 0));
+    const int64_t c0 = k * per, cnt = std::min(per, C - c0);
+    rc = drain_to_host(A, S.cs, S.buf[b], (double*)(dst + (uint64_t)c0 * R), (uint64_t)cnt * R, false);
+    if (rc) return rc;
+    CU(A->cuEventRecord(S.ev[b][1], S.cs));
+  }
+  CU(A->cuStreamSynchronize(S.cs));
+  CU(A->cuStreamSynchronize(s->stream));
+  return RN_OK;
+}
+
+// records at src -> chains [c_begin, c_begin + count): the upload of chunk k + 1 on the copy stream overlaps rn_k_state_unpack of
+// chunk k on the sampler's stream
+int ckpt_load_records(const Api* A, rn_sampler* s, const std::vector<CkptField>& L, uint64_t R, const uint8_t* src, int64_t count,
+                      int64_t c_begin) {
+  const StateModule* M = nullptr;
+  int rc = state_module(A, s->m->device, &M);
+  if (rc) return rc;
+  const int64_t per = (int64_t)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)count, ckpt_stage_bytes() / R));
+  const int64_t chunks = (count + per - 1) / per;
+  CkptStaging S{A};
+  rc = S.init((uint64_t)per * R, chunks > 1 ? 2 : 1);
+  if (rc) return rc;
+  RnStateArgs a = ckpt_args(s, L, R);
+  for (int64_t k = 0; k < chunks; k++) {
+    const int b = (int)(k & 1);
+    const int64_t c0 = k * per, cnt = std::min(per, count - c0);
+    if (S.used[b]) CU(A->cuStreamWaitEvent(S.cs, S.ev[b][1], 0));  // its previous chunk has been unpacked
+    CU(A->cuMemcpyHtoDAsync(S.buf[b], src + (uint64_t)c0 * R, (uint64_t)cnt * R, S.cs));
+    CU(A->cuEventRecord(S.ev[b][0], S.cs));
+    CU(A->cuStreamWaitEvent(s->stream, S.ev[b][0], 0));
+    a.c0 = c_begin + c0;
+    a.count = cnt;
+    a.staging = (unsigned*)(uintptr_t)S.buf[b];
+    rc = state_launch(A, M->unpack, a, s->stream);
+    if (rc) return rc;
+    CU(A->cuEventRecord(S.ev[b][1], s->stream));
+    S.used[b] = true;
+  }
+  CU(A->cuStreamSynchronize(s->stream));
+  return RN_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int rn_sampler_save(rn_sampler* s, void* buf, size_t cap, size_t* needed) {
+  if (!s) return fail(RN_E_INVALID, "null sampler");
+  std::lock_guard<std::recursive_mutex> model_lock_(s->m->mu);
+  std::string why;
+  const Api* A = api(&why);
+  if (!A) return fail(RN_E_CUDA, why);
+  CU(A->cuCtxSetCurrent(s->m->ctx));
+  CU(A->cuStreamSynchronize(s->stream));
+  int rc = close_sampling_span(A, s);  // the device time so far is part of the checkpoint
+  if (rc) return rc;
+  uint64_t R = 0;
+  const std::vector<CkptField> L = ckpt_layout(s, &R);
+  rn_ckpt_header h;
+  ckpt_header(s, L, R, h);
+  const uint64_t table_off = sizeof(h), rep_off = table_off + L.size() * sizeof(rn_ckpt_field), rec_off = rep_off + h.step_bytes + h.pool_bytes,
+                 total = rec_off + (uint64_t)s->chains * R + 8;
+  if (needed) *needed = (size_t)total;
+  if (!buf) return RN_OK;
+  if (cap < total) return fail(RN_E_INVALID, "rn_sampler_save: buffer of " + std::to_string(cap) + " bytes, the checkpoint needs " + std::to_string(total));
+  rc = model_fingerprint(A, s->m, &h.fingerprint);
+  if (rc) return rc;
+  uint8_t* p = (uint8_t*)buf;
+  std::memcpy(p, &h, sizeof(h));
+  for (size_t f = 0; f < L.size(); f++) std::memcpy(p + table_off + f * sizeof(rn_ckpt_field), &L[f].f, sizeof(rn_ckpt_field));
+  CU(A->cuMemcpyDtoH(p + rep_off, s->d_step, h.step_bytes));
+  CU(A->cuMemcpyDtoH(p + rep_off + h.step_bytes, s->d_pool, h.pool_bytes));
+  rc = ckpt_save_records(A, s, L, R, p + rec_off);
+  if (rc) return rc;
+  const uint64_t sum = blob_hash(p, total - 8);
+  std::memcpy(p + total - 8, &sum, 8);
+  return RN_OK;
+}
+
+int rn_sampler_restore(rn_model* m, const rn_config* cfg, const void* const* blobs, const size_t* lens, int n_blobs, rn_sampler** out) {
+  if (!m || !cfg || !blobs || !lens || n_blobs < 1 || !out) return fail(RN_E_INVALID, "null argument");
+  std::lock_guard<std::recursive_mutex> model_lock_(m->mu);
+  if (cfg->struct_size != (int32_t)sizeof(rn_config)) return fail(RN_E_INVALID, "rn_config.struct_size mismatch");
+  std::vector<CkptView> V((size_t)n_blobs);
+  int64_t chains = 0;
+  for (int i = 0; i < n_blobs; i++) {
+    const std::string what = "rn_sampler_restore: checkpoint " + std::to_string(i);
+    int rc = ckpt_parse(blobs[i], lens[i], what, &V[i]);
+    if (rc) return rc;
+    if (i > 0) {
+      rc = ckpt_same(V[0], V[i], what);
+      if (rc) return rc;
+    }
+    chains += V[i].h.chains;
+  }
+  const rn_ckpt_header& h0 = V[0].h;
+  if (n_blobs > 1 && !ckpt_independent(h0))
+    return fail(RN_E_INVALID, "rn_sampler_restore: checkpoints taken during a pooled warmup cannot be concatenated (pooled windows sum "
+                              "per rank, so their bits depend on how the chains are split)");
+  for (int i = 0; i + 1 < n_blobs; i++)
+    if (h0.mma && h0.mma_chains > 0 && V[i].h.chains % h0.mma_chains != 0)
+      return fail(RN_E_INVALID, "rn_sampler_restore: on the DMMA path every checkpoint but the last must hold a multiple of " +
+                                    std::to_string(h0.mma_chains) + " chains");
+  if (chains > INT32_MAX) return fail(RN_E_INVALID, "rn_sampler_restore: too many chains");
+  if (h0.n != (int64_t)m->n_params)
+    return fail(RN_E_INVALID, "rn_sampler_restore: n differs (checkpoint " + std::to_string(h0.n) + ", model " + std::to_string(m->n_params) + ")");
+  int rc = ckpt_config_matches(h0, *cfg);
+  if (rc) return rc;
+  if (m->device < 0) return fail(RN_E_CUDA, "model was created without a device (no CPU fallback)");
+  std::string why;
+  const Api* A = api(&why);
+  if (!A) return fail(RN_E_CUDA, why);
+  CU(A->cuCtxSetCurrent(m->ctx));
+  uint64_t fp = 0;
+  rc = model_fingerprint(A, m, &fp);
+  if (rc) return rc;
+  if (fp != h0.fingerprint) return fail(RN_E_INVALID, "rn_sampler_restore: the model differs from the checkpoint's (fingerprint of its RIR and data)");
+  rn_config c = *cfg;
+  c.warmup_iterations = h0.warmup_iterations;  // (equal unless warmup has finished: then the checkpoint's count is the one run)
+  c.rng_states = nullptr;
+  std::vector<int64_t> seeds((size_t)chains, 0);  // every chain's state is overwritten below
+  rn_sampler* raw = nullptr;
+  rc = rn_sampler_create(m, &c, seeds.data(), (int)chains, &raw);
+  if (rc) return rc;
+  struct Destroy {
+    void operator()(rn_sampler* p) const { rn_sampler_destroy(p); }
+  };
+  std::unique_ptr<rn_sampler, Destroy> s(raw);
+  {  // the resolved shape must be the checkpoint's; the warp-per-chain placement may differ (it is memory, not arithmetic)
+    rn_ckpt_header now;
+    uint64_t R_now = 0;
+    ckpt_header(s.get(), ckpt_layout(s.get(), &R_now), R_now, now);
+#define RN_CKPT_SHAPE(f) \
+  if (now.f != h0.f) return fail(RN_E_INVALID, "rn_sampler_restore: kernel shape: " #f " differs (checkpoint " + std::to_string(h0.f) + ", here " + std::to_string(now.f) + ")");
+    RN_CKPT_SHAPE(backend) RN_CKPT_SHAPE(wpc_k) RN_CKPT_SHAPE(mma) RN_CKPT_SHAPE(mma_chains) RN_CKPT_SHAPE(mass_max)
+    RN_CKPT_SHAPE(adjoint) RN_CKPT_SHAPE(fast) RN_CKPT_SHAPE(ehmc) RN_CKPT_SHAPE(step_pool) RN_CKPT_SHAPE(mass_pool)
+    RN_CKPT_SHAPE(step_bytes) RN_CKPT_SHAPE(pool_bytes)
+#undef RN_CKPT_SHAPE
+  }
+  s->initialized = h0.initialized != 0;
+  s->warm_done = h0.warm_done;
+  s->stats_reset_for_sampling = h0.stats_reset_for_sampling != 0;
+  s->win_size = h0.win_size, s->win_i = h0.win_i, s->win_j = h0.win_j, s->est_samples = h0.est_samples, s->mass_kind = h0.mass_kind;
+  s->chain_offset = h0.chain_offset;
+  for (const CkptView& v : V) {  // chains that ran side by side: the longest device time
+    s->sampling_ms = std::max(s->sampling_ms, v.h.sampling_ms);
+    s->track_ms = std::max(s->track_ms, v.h.track_ms);
+    s->sampling_iterations = std::max(s->sampling_iterations, v.h.sampling_iterations);
+  }
+  if (h0.track) {
+    rc = track_alloc(A, s.get());
+    if (rc) return rc;
+    s->track = true;
+    s->track_thin = h0.track_thin;
+    s->track_seen = h0.track_seen;
+    s->track_kept = h0.track_kept;
+  }
+  uint64_t R = 0;
+  const std::vector<CkptField> L = ckpt_layout(s.get(), &R);
+  bool same = L.size() == V[0].table.size() && R == h0.record_bytes;
+  for (size_t f = 0; same && f < L.size(); f++) same = std::memcmp(&L[f].f, &V[0].table[f], sizeof(rn_ckpt_field)) == 0;
+  if (!same) return fail(RN_E_INVALID, "rn_sampler_restore: the checkpoint's record layout differs from this sampler's");
+  CU(A->cuMemcpyHtoD(s->d_step, V[0].p + V[0].rep_off, h0.step_bytes));
+  CU(A->cuMemcpyHtoD(s->d_pool, V[0].p + V[0].rep_off + h0.step_bytes, h0.pool_bytes));
+  int64_t at = 0;
+  for (const CkptView& v : V) {
+    rc = ckpt_load_records(A, s.get(), L, R, v.p + v.rec_off, v.h.chains, at);
+    if (rc) return rc;
+    at += v.h.chains;
+  }
+  *out = s.release();
+  return RN_OK;
+}
+
+int rn_checkpoint_info(const void* blob, size_t len, struct rn_checkpoint_info* out) {
+  if (!out) return fail(RN_E_INVALID, "null argument");
+  CkptView v;
+  int rc = ckpt_parse(blob, len, "rn_checkpoint_info", &v);
+  if (rc) return rc;
+  const rn_ckpt_header& h = v.h;
+  std::memset(out, 0, sizeof(*out));
+  out->version = (int32_t)h.version;
+  out->phase = !h.initialized ? 0 : (h.warm_done < h.warmup_iterations ? 1 : (h.stats_reset_for_sampling ? 3 : 2));
+  out->n = h.n, out->chains = h.chains, out->chain_offset = h.chain_offset;
+  out->warmup_iterations = h.warmup_iterations, out->warm_done = h.warm_done;
+  out->win_size = h.win_size, out->win_i = h.win_i, out->win_j = h.win_j, out->est_samples = h.est_samples;
+  out->mass_kind = h.mass_kind, out->track = h.track, out->track_thin = h.track_thin;
+  out->track_seen = h.track_seen, out->track_kept = h.track_kept;
+  out->backend = h.backend, out->wpc_k = h.wpc_k, out->mma = h.mma, out->wpc_place = h.wpc_place;
+  out->fingerprint = h.fingerprint;
+  out->header_bytes = v.table_off, out->table_bytes = v.rep_off - v.table_off, out->replicated_bytes = v.rec_off - v.rep_off;
+  out->record_bytes = h.record_bytes, out->records_bytes = (uint64_t)h.chains * h.record_bytes, out->total_bytes = v.total;
+  return RN_OK;
+}
+
+int rn_checkpoint_slice(const void* blob, size_t len, int64_t begin, int64_t end, void* out, size_t cap, size_t* needed) {
+  CkptView v;
+  int rc = ckpt_parse(blob, len, "rn_checkpoint_slice", &v);
+  if (rc) return rc;
+  const rn_ckpt_header& h = v.h;
+  if (begin < 0 || end <= begin || end > h.chains)
+    return fail(RN_E_INVALID, "rn_checkpoint_slice: chains [" + std::to_string(begin) + ", " + std::to_string(end) + ") of " + std::to_string(h.chains));
+  if ((begin > 0 || end < h.chains) && !ckpt_independent(h))
+    return fail(RN_E_INVALID, "rn_checkpoint_slice: a checkpoint taken during a pooled warmup cannot be sliced (pooled windows sum per rank, "
+                              "so their bits depend on how the chains are split)");
+  if (!ckpt_mma_aligned(h, begin, end))
+    return fail(RN_E_INVALID, "rn_checkpoint_slice: on the DMMA path a slice must start at a multiple of " + std::to_string(h.mma_chains) +
+                              " chains and end at the last chain or after a multiple of it");
+  const uint64_t total = v.rec_off + (uint64_t)(end - begin) * h.record_bytes + 8;
+  if (needed) *needed = (size_t)total;
+  if (!out) return RN_OK;
+  if (cap < total) return fail(RN_E_INVALID, "rn_checkpoint_slice: buffer of " + std::to_string(cap) + " bytes, the slice needs " + std::to_string(total));
+  uint8_t* p = (uint8_t*)out;
+  rn_ckpt_header nh = h;
+  nh.chains = end - begin;
+  nh.chain_offset = h.chain_offset + begin;
+  std::memcpy(p, &nh, sizeof(nh));
+  std::memcpy(p + v.table_off, v.p + v.table_off, v.rec_off - v.table_off);
+  std::memcpy(p + v.rec_off, v.p + v.rec_off + (uint64_t)begin * h.record_bytes, (uint64_t)(end - begin) * h.record_bytes);
+  const uint64_t sum = blob_hash(p, total - 8);
+  std::memcpy(p + total - 8, &sum, 8);
   return RN_OK;
 }
 

@@ -13,6 +13,8 @@ with the dense tuner the n^2 sums of C2_c[j][k] + L d_c[j] d_c[k] (`combine_welf
 
 torch.distributed is used purely as plumbing (NCCL on GPUs, gloo in the CPU tests).
 """
+import os
+
 import numpy as np
 
 
@@ -179,3 +181,22 @@ def best_start(x, f, info=None, group=None):
     dist.all_gather_object(pieces, mine, group=group)
     owner = min(range(world), key=lambda r: (pieces[r][0], r))
     return pieces[owner][1], pieces[owner][0], owner
+
+
+def save_rank_checkpoint(sampler, directory, group=None):
+    """rn_sampler_save on every rank: rank r writes its sampler's checkpoint to <directory>/rank<r>.ckpt (written to a temporary
+    name, then renamed, so a lost process leaves the previous file whole) and the ranks meet at a barrier.  The files of all
+    ranks, restored in rank order with CudaSampler.restore(model, config, [blobs]), are the job's chains in their global order;
+    a resumed job may use fewer or more GPUs (checkpoint_slice re-cuts the chains) once warmup has finished, or at any phase
+    with per-chain adaptation.  Returns the path."""
+    import torch.distributed as dist
+    rank = dist.get_rank(group) if dist.is_available() and dist.is_initialized() else 0
+    path = os.path.join(directory, "rank%d.ckpt" % rank)
+    with open(path + ".tmp", "wb") as f:
+        f.write(sampler.save())
+        f.flush()
+        os.fsync(f.fileno())
+    os.replace(path + ".tmp", path)
+    if dist.is_available() and dist.is_initialized():
+        dist.barrier(group)
+    return path

@@ -122,6 +122,20 @@ object CudaSampling {
     s
   }
 
+  /** Checkpoint of a staged sampler (rn_sampler_save, DESIGN.md 3.6): its whole state in page-locked memory (one DMA per
+    * chunk), to be written to a file or restored in another process or on another device.  Free with Native.hostFree. */
+  def save(sampler: Long, device: Int = 0): ByteBuffer = {
+    val buf = Native.hostAlloc(device, Native.samplerSave(sampler, null))
+    Native.samplerSave(sampler, buf)
+    buf
+  }
+
+  /** rn_sampler_restore: a staged sampler (handle) that continues the blobs' chains, concatenated in order, with the same bits
+    * as the uninterrupted run.  `config` must agree with the checkpoints' semantic fields; `iterations` may grow, so that a
+    * finished run can be extended.  Each blob's bytes are its limit. */
+  def restore(model: Long, config: SamplerConfig, blobs: Seq[ByteBuffer]): Long =
+    Native.samplerRestore(model, lower(config), blobs.toArray, blobs.map(_.limit.toLong).toArray)
+
   /** `Model.density()` for API completeness (Optimizer.lbfgs, JMH): one crossing per update -- NOT the fast path. */
   def density(model: Model, device: Int = 0): DensityFunction = {
     val cm = CudaCompiler.compileTargets(model.targetGroup, withGradient = false, device = device)

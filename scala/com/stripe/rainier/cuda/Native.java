@@ -77,5 +77,18 @@ public final class Native {
    *  of an attached communicator calls it) */
   public static native void samplerTrackedDiagnostics(long sampler, double[] out);
 
+  /** rn_sampler_save: the staged sampler's whole state into a direct ByteBuffer (page-locked memory from hostAlloc is written by
+   *  DMA); out == null returns the size only.  Returns the checkpoint's bytes */
+  public static native long samplerSave(long sampler, ByteBuffer out);
+
+  /** rn_sampler_restore: a new staged sampler whose chains are the blobs' chains, concatenated in order (lens: bytes of each) */
+  public static native long samplerRestore(long model, ByteBuffer config, ByteBuffer[] blobs, long[] lens);
+
+  /** rn_checkpoint_info, no device: out = [version, phase, n, chains, chainOffset, warmDone, trackKept, totalBytes] */
+  public static native void checkpointInfo(ByteBuffer blob, long len, long[] out);
+
+  /** rn_checkpoint_slice, no device: chains [begin, end) as a checkpoint of their own; out == null returns the size only */
+  public static native long checkpointSlice(ByteBuffer blob, long len, long begin, long end, ByteBuffer out);
+
   public static native String lastError();
 }
