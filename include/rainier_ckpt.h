@@ -5,7 +5,10 @@
  *   1. rn_ckpt_header                                  (header_bytes)
  *   2. n_fields x rn_ckpt_field                        the record layout: fields in record order
  *   3. step_bytes: d_step, int64 [2 + warmup] with pooled step-size adaptation, else [1]; then
- *      pool_bytes: the pooled window buffer (doubles)   -- both shared by all chains, copied as they are
+ *      pool_bytes: the pooled window buffer (doubles)   -- both shared by all chains, copied as they are; then
+ *      reserved1 bytes: with pooled trajectory lengths (reserved0 = rn_config.trajectory_adaptation = RN_ADAPT_POOLED) the
+ *      pooled histogram, int64 [max_steps + 1], once the first sampling launch has built it (0 bytes before, and always
+ *      with per-chain lengths: such blobs are laid out exactly as without the extension)
  *   4. chains x record_bytes                           chain-major records: chain c's fields in table order, each its
  *                                                      elements back to back (8-byte fields first, then 4-byte ones,
  *                                                      padded to a multiple of 8 bytes)
@@ -69,7 +72,8 @@ typedef struct rn_ckpt_header {
   int32_t initial_window_size, skip_first, skip_last, static_matrix, adaptation, math_mode, gradient_mode, stats_window,
       warmup_iterations, iterations;
   /* the resolved kernel shape (wpc_place is informational: a restore may use another placement) */
-  int32_t backend, wpc_k, mma, mma_chains, wpc_place, mass_max, adjoint, fast, ehmc, step_pool, mass_pool, reserved0;
+  int32_t backend, wpc_k, mma, mma_chains, wpc_place, mass_max, adjoint, fast, ehmc, step_pool, mass_pool,
+          reserved0;  /* rn_config.trajectory_adaptation */
   int64_t n, chains, chain_offset; /* chain_offset: index of the first chain in the sampler that was saved */
   /* the sampler's host mirror */
   int32_t initialized, warm_done, stats_reset_for_sampling, win_size, win_i, win_j, est_samples, mass_kind;
@@ -79,7 +83,7 @@ typedef struct rn_ckpt_header {
   /* accumulated device times */
   double sampling_ms, track_ms;
   int64_t sampling_iterations;
-  uint32_t n_fields, reserved1;
+  uint32_t n_fields, reserved1;  /* reserved1: bytes of the pooled trajectory-length histogram (part 3) */
   uint64_t step_bytes, pool_bytes, record_bytes;
 } rn_ckpt_header;
 

@@ -109,7 +109,20 @@ typedef struct rn_config {
   int32_t skip_first;        /* default 50 */
   int32_t skip_last;         /* default 50 */
   int32_t static_matrix;     /* RN_MATRIX_* when mass_tuner == RN_MASS_STATIC */
-  int32_t reserved2;
+  int32_t trajectory_adaptation; /* extension, EHMCSampler only: RN_ADAPT_PER_CHAIN (parity with the reference, default: every
+                                sampling iteration of a chain draws its length from its own ring of U-turn counts) or
+                                RN_ADAPT_POOLED: warmup is unchanged; at the first sampling launch the histogram h[0..max_steps]
+                                (int64) counts, over every chain (and, with a communicator attached, every rank), the ring
+                                entries steps.sample() chooses from -- indices [0, ring_full ? buf_size : ring_i + 1), so a
+                                ring that never filled offers slot 0, whose value is 0 -- and sampling iteration t (0 = the
+                                first after warmup) of EVERY chain takes L_t leapfrog steps:
+                                  T = sum h;  c[l] = h[0] + ... + h[l];  F = the 64-bit fingerprint of the counts (the
+                                  checkpoints' word hash, rn_trajectory_lengths_sequence);
+                                  z = splitmix64(F + (t + 1) * 0x9E3779B97F4A7C15), the finaliser z ^= z >> 30,
+                                  z *= 0xBF58476D1CE4E5B9, z ^= z >> 27, z *= 0x94D049BB133111EB, z ^= z >> 31 (mod 2^64);
+                                  r = mulhi64(z, T);  L_t = min { l : c[l] > r }.
+                                No chain's RNG is consumed.  The first rn_sampler_run after warmup is a collective when a
+                                communicator is attached.  max_steps <= 65536 in this mode */
   const double* static_matrix_elements; /* n (diagonal) or n*n (dense) doubles, shared by all chains */
 
   /* extensions (not in the reference) */
@@ -264,6 +277,13 @@ int rn_sampler_set_comm(rn_sampler* s, rn_comm* comm);
 /* the collective of this path: ncclAllReduce calls issued by the pooled warmup so far and their summed device time in
  * microseconds (event pairs on the sampler's stream; synchronises it) */
 int rn_sampler_comm_stats(rn_sampler* s, int64_t* calls, double* total_us);
+/* pooled trajectory lengths (rn_config.trajectory_adaptation == RN_ADAPT_POOLED): the pooled histogram h[0..max_steps] over
+ * every chain of every rank.  *n = max_steps + 1; counts (may be NULL) receives min(cap, *n) of them.  RN_E_INVALID in
+ * per-chain mode and before the first sampling launch has built the histogram. */
+int rn_sampler_trajectory_lengths(rn_sampler* s, int64_t* counts, int cap, int* n);
+/* tooling / tests (no device): L_t of rn_config.trajectory_adaptation for t = t0 .. t0 + count - 1 given the histogram
+ * counts[0..bins) (bins <= 65537, every count >= 0, a positive total) */
+int rn_trajectory_lengths_sequence(const int64_t* counts, int bins, int64_t t0, int64_t count, int32_t* out);
 void rn_sampler_destroy(rn_sampler* s);
 
 /* ---- checkpoints of a staged sampler (byte format: rainier_ckpt.h; DESIGN.md 3.6) --------------------------------- */
@@ -278,7 +298,7 @@ void rn_sampler_destroy(rn_sampler* s);
  * rn_sampler_create builds them for `cfg`.  RN_E_INVALID, naming the first differing item, when: a blob is truncated,
  * corrupted (checksum) or of another version; the model (fingerprint of its RIR and data) or n differs; a semantic
  * config field differs (sampler and its parameters, the tuners and their parameters, adaptation, step_adaptation,
- * math_mode, gradient_mode, stats_window, and warmup_iterations while warmup is unfinished); the resolved kernel shape
+ * trajectory_adaptation, math_mode, gradient_mode, stats_window, and warmup_iterations while warmup is unfinished); the resolved kernel shape
  * differs (the warp-per-chain placement may); several blobs disagree, or are concatenated where chains are not independent
  * (pooled adaptation before the end of warmup).  iterations, launch_iterations and the device may differ.
  * rn_checkpoint_info / rn_checkpoint_slice need no device.  A slice is chains [begin, end) as a blob of its own; refused

@@ -281,6 +281,17 @@ JNIEXPORT void JNICALL Java_com_stripe_rainier_cuda_Native_samplerTrackedDiagnos
   if (rn_sampler_tracked_diagnostics((rn_sampler*)(intptr_t)s, vo.data()) != RN_OK) return throw_last(env);
   out_doubles(env, out, vo.data(), vo.size());
 }
+// def samplerTrajectoryLengths(sampler: Long, counts: Array[Long] /* or null: size only */): Int   (bins = maxSteps + 1)
+JNIEXPORT jint JNICALL Java_com_stripe_rainier_cuda_Native_samplerTrajectoryLengths(JNIEnv* env, jclass, jlong s, jlongArray counts) {
+  int n = 0;
+  if (rn_sampler_trajectory_lengths((rn_sampler*)(intptr_t)s, nullptr, 0, &n) != RN_OK) return throw_last(env), 0;
+  if (counts) {
+    std::vector<int64_t> v((size_t)n);
+    if (rn_sampler_trajectory_lengths((rn_sampler*)(intptr_t)s, v.data(), n, &n) != RN_OK) return throw_last(env), 0;
+    env->SetLongArrayRegion(counts, 0, std::min<jsize>(env->GetArrayLength(counts), (jsize)n), (const jlong*)v.data());
+  }
+  return (jint)n;
+}
 // ---- checkpoints of a staged sampler (rn_sampler_save / rn_sampler_restore); blobs travel in direct ByteBuffers ----
 // def samplerSave(sampler: Long, out: ByteBuffer /* direct, or null: size only */): Long   (bytes of the checkpoint)
 JNIEXPORT jlong JNICALL Java_com_stripe_rainier_cuda_Native_samplerSave(JNIEnv* env, jclass, jlong s, jobject out) {

@@ -45,7 +45,7 @@ class Config(C.Structure):
         ("skip_first", C.c_int32),
         ("skip_last", C.c_int32),
         ("static_matrix", C.c_int32),
-        ("reserved2", C.c_int32),
+        ("trajectory_adaptation", C.c_int32),
         ("static_matrix_elements", C.POINTER(C.c_double)),
         ("adaptation", C.c_int32),
         ("math_mode", C.c_int32),

@@ -83,6 +83,8 @@ def lib():
         L.rn_sampler_read_trace.argtypes = [C.c_void_p, C.c_void_p]
         L.rn_sampler_set_comm.argtypes = [C.c_void_p, C.c_void_p]
         L.rn_sampler_comm_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_double)]
+        L.rn_sampler_trajectory_lengths.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
+        L.rn_trajectory_lengths_sequence.argtypes = [C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_void_p]
         L.rn_comm_unique_id.argtypes = [C.c_char_p]
         L.rn_comm_create.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
         L.rn_comm_destroy.argtypes = [C.c_void_p]
@@ -275,6 +277,8 @@ class SamplerConfig:
     gradientMode = abi.RN_GRAD_AUTO
     adaptation = abi.RN_ADAPT_PER_CHAIN
     stepAdaptation = abi.RN_ADAPT_PER_CHAIN  # RN_ADAPT_POOLED: one DualAvg step size fitted to all chains' mean acceptance
+    trajectoryAdaptation = abi.RN_ADAPT_PER_CHAIN  # RN_ADAPT_POOLED (EHMC): every chain samples with one shared length per
+                                                    # iteration, drawn from the U-turn counts of all chains' warmups
     launchIterations = 0
     backend = abi.RN_BACKEND_AUTO
 
@@ -340,6 +344,7 @@ def lower_config(config):
     c.math_mode, c.gradient_mode = int(config.mathMode), int(config.gradientMode)
     c.adaptation, c.launch_iterations = int(config.adaptation), int(config.launchIterations)
     c.step_adaptation = int(config.stepAdaptation)
+    c.trajectory_adaptation = int(config.trajectoryAdaptation)
     c.backend = int(config.backend)
     return c, keep
 
@@ -851,6 +856,15 @@ def checkpoint_info(blob):
     return {f: getattr(info, f) for f, _ in abi.CheckpointInfo._fields_ if f != "reserved"}
 
 
+def trajectory_lengths_sequence(counts, t0, count):
+    """tooling / tests (no device): rn_trajectory_lengths_sequence -- L_t of pooled trajectory lengths for t = t0 .. t0 + count - 1
+    given the pooled histogram `counts` (the definition is in rainier_cuda.h, rn_config.trajectory_adaptation)"""
+    h = np.ascontiguousarray(counts, dtype=np.int64)
+    out = np.zeros(int(count), dtype=np.int32)
+    _check(lib().rn_trajectory_lengths_sequence(h.ctypes.data, len(h), int(t0), int(count), out.ctypes.data))
+    return out
+
+
 def checkpoint_slice(blob, begin, end):
     """rn_checkpoint_slice: chains [begin, end) of a checkpoint as a checkpoint of their own (bytearray; no device needed)"""
     a = _blob_view(blob)
@@ -893,6 +907,15 @@ class CudaSampler:
         calls, us = C.c_int64(0), C.c_double(0.0)
         _check(lib().rn_sampler_comm_stats(self.h, C.byref(calls), C.byref(us)))
         return int(calls.value), float(us.value)
+
+    def trajectory_lengths(self):
+        """the pooled histogram of U-turn counts over every chain of every rank, int64 [max_steps + 1]
+        (trajectoryAdaptation = RN_ADAPT_POOLED, after the first sampling launch)"""
+        n = C.c_int(0)
+        _check(lib().rn_sampler_trajectory_lengths(self.h, None, 0, C.byref(n)))
+        out = np.zeros(n.value, dtype=np.int64)
+        _check(lib().rn_sampler_trajectory_lengths(self.h, out.ctypes.data, n.value, C.byref(n)))
+        return out
 
     def warmup(self, iterations=-1):
         _check(lib().rn_sampler_warmup(self.h, int(iterations)))

@@ -61,6 +61,16 @@ struct RnArgs {
   // warp-per-chain modules with RN_WPC_PLACE > 0 (rn_sampler_wpc.cuh): the chains' state slices that do not fit shared memory,
   // [chain][RN_WPC_GLOBAL_DOUBLES]; NULL otherwise
   double* wpc_state;
+  // pooled trajectory lengths (RN_TRAJ_POOL modules only, rn_sampler_common.cuh): the inclusive prefix sums c[0..traj_bins) of
+  // the pooled histogram of U-turn counts, its total T = c[traj_bins - 1] and fingerprint F, and the sampling iteration t of
+  // this launch's first iteration; rn_k_traj_hist counts the chains' rings into traj_hist
+  const rn_i64* traj_cum;
+  rn_i64* traj_hist;
+  rn_i64 traj_total;
+  rn_i64 traj_fp;
+  rn_i64 traj_t0;
+  int traj_bins;
+  int pad2;
 };
 
 // argument block of rn_k_eval (rn_function.cuh): batched evaluation of a compiled function, generic addressing

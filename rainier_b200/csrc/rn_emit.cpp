@@ -1968,6 +1968,7 @@ std::string emit_source(const Program& P, const EmitOptions& opt) {
   os << "#define RN_ENABLE_EHMC " << (opt.enable_ehmc ? 1 : 0) << "\n";
   if (opt.step_pool) os << "#define RN_STEP_POOL 1\n";
   if (opt.mass_pool) os << "#define RN_MASS_POOL 1\n";
+  if (opt.traj_pool) os << "#define RN_TRAJ_POOL 1\n";
   if (opt.fast_math) os << "#define RN_FAST_MATH 1\n";
   if (opt.backend == 0) os << "#define RN_TS_RESTORE " << (opt.tpc_restore ? 1 : 0) << "\n";
   if (opt.backend == 1) {

@@ -15,6 +15,7 @@ struct EmitOptions {
   bool enable_ehmc = false;
   bool step_pool = false; // pooled step-size adaptation (rn_sampler_common.cuh): RN_STEP_POOL kernels
   bool mass_pool = false; // pooled dense mass windows (rn_sampler_common.cuh): RN_MASS_POOL kernels
+  bool traj_pool = false; // pooled EHMC trajectory lengths (rn_sampler_common.cuh): RN_TRAJ_POOL kernels
   bool tpc_restore = false; // thread per chain: the iteration's restore point in shared memory (RN_TS_RESTORE, rn_sampler.cuh)
   int tma_stages = 0;     // warp per chain: shared-memory stages of the CTA-shared data-tile pipeline (0 = off)
   int wpc_k = 1;          // warp per chain: warps owning one chain (1, 2, 4 or 8; > 1 for chains with a large state)

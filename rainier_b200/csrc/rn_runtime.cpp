@@ -158,9 +158,10 @@ struct KernelKey {
   int block = 0;  // thread-per-chain: CTA size the module was compiled for (RN_BLOCK_DIM), 0 = any (emit / density-only uses)
   bool step_pool = false;  // pooled step-size adaptation compiled in (RN_STEP_POOL)
   bool mass_pool = false;  // pooled dense mass windows compiled in (RN_MASS_POOL)
+  bool traj_pool = false;  // pooled EHMC trajectory lengths compiled in (RN_TRAJ_POOL)
   bool operator<(const KernelKey& o) const {
-    return std::tie(adjoint, fast, ehmc, mass_max, backend, block, step_pool, mass_pool) <
-           std::tie(o.adjoint, o.fast, o.ehmc, o.mass_max, o.backend, o.block, o.step_pool, o.mass_pool);
+    return std::tie(adjoint, fast, ehmc, mass_max, backend, block, step_pool, mass_pool, traj_pool) <
+           std::tie(o.adjoint, o.fast, o.ehmc, o.mass_max, o.backend, o.block, o.step_pool, o.mass_pool, o.traj_pool);
   }
 };
 // SMs of a device; handles without one (emit / compile only) assume an H100 SXM's 132
@@ -207,6 +208,8 @@ struct Kernel {
   int backend = 0;            // 0 thread per chain, 1 warp per chain
   bool step_pool = false;     // rn_k_step_pool compiled in (pooled step-size adaptation)
   bool mass_pool = false;     // rn_k_pool_reduce_dense / rn_k_pool_factor / rn_k_pool_apply_dense compiled in (pooled dense windows)
+  bool traj_pool = false;     // rn_k_traj_hist compiled in (pooled trajectory lengths)
+  CUfunction k_traj_hist = nullptr;
   unsigned tpc_block = 0;     // backend 0: the CTA size this module was compiled for (0: reads blockDim.x)
   int wpc_smem_doubles = 0;   // per-warp dynamic shared memory (backend 1)
   int wpc_place = 0;          // backend 1: RN_WPC_PLACE, where a chain's state lives (rn_sampler_wpc.cuh)
@@ -299,6 +302,7 @@ static KernelKey key_for(const rn_model* m, const rn_config* cfg) {
   k.ehmc = cfg && cfg->sampler == RN_SAMPLER_EHMC;
   k.step_pool = cfg && cfg->step_adaptation == RN_ADAPT_POOLED;
   k.mass_pool = cfg && cfg->adaptation == RN_ADAPT_POOLED && cfg->mass_tuner == RN_MASS_DENSE;
+  k.traj_pool = k.ehmc && cfg->trajectory_adaptation == RN_ADAPT_POOLED;
   k.mass_max = 0;
   if (cfg) {
     if (cfg->mass_tuner == RN_MASS_DIAGONAL) k.mass_max = 1;
@@ -400,6 +404,7 @@ static int get_kernel(rn_model* m, const rn_config* cfg, Kernel** out, std::stri
   eo.enable_ehmc = key.ehmc;
   eo.step_pool = key.step_pool;
   eo.mass_pool = key.mass_pool;
+  eo.traj_pool = key.traj_pool;
   eo.target_base = m->target_base;
   eo.target_pitch = m->target_pitch;
   if (eo.backend == 1 && P->symbolic && P->n_params > 96)
@@ -407,6 +412,7 @@ static int get_kernel(rn_model* m, const rn_config* cfg, Kernel** out, std::stri
   K->backend = eo.backend;
   K->step_pool = key.step_pool;
   K->mass_pool = key.mass_pool;
+  K->traj_pool = key.traj_pool;
   K->tpc_block = (unsigned)key.block;
   if (eo.backend == 0) {  // rn_sampler.cuh: RN_TS_DOUBLES * 8 + RN_TS_INTS * 4
     const unsigned n = P->n_params;
@@ -464,9 +470,10 @@ static int get_kernel(rn_model* m, const rn_config* cfg, Kernel** out, std::stri
     const size_t left = cap - (size_t)stages * tile - (stages ? 256 : 0);
     K->warps_per_cta = (int)std::max<size_t>(1, std::min<size_t>((size_t)wmax, left / std::max<size_t>(per_warp, 1)));
     eo.tma_stages = stages;
-    // chain-batched fp64 tensor-core path (rn_emit.cpp: Emitter::mma_block): HMC (every chain of a CTA evaluates the density
-    // equally often), not the dense-mass code, one warp per chain, 8 chains per CTA, and every streamed target eligible
-    bool want_mma = !key.ehmc && key.mass_max < 2 && eo.wpc_k == 1 && eo.wpc_place == 0 && z.mma_ok && !P->symbolic;
+    // chain-batched fp64 tensor-core path (rn_emit.cpp: Emitter::mma_block): HMC or the sampling phase of EHMC with pooled
+    // trajectory lengths (every chain of a CTA evaluates the density equally often; such a module's warmup launches run with
+    // a.tma = 0, run_phase), not the dense-mass code, one warp per chain, 8 chains per CTA, and every streamed target eligible
+    bool want_mma = (!key.ehmc || key.traj_pool) && key.mass_max < 2 && eo.wpc_k == 1 && eo.wpc_place == 0 && z.mma_ok && !P->symbolic;
     if (const char* e = getenv("RN_MMA")) want_mma = want_mma && atoi(e) != 0;
     if (want_mma) {
       // 16 chains per CTA when they fit (two chain groups whose warps pair up on a dot's column block: twice the warps per
@@ -627,6 +634,7 @@ static int load_kernel(const Api* A, rn_model* m, Kernel* K) {
   CU(A->cuModuleGetFunction(&K->k_diag_accum, K->mod, "rn_k_diag_accum"));
   CU(A->cuModuleGetFunction(&K->k_diag_terms, K->mod, "rn_k_diag_terms"));
   if (K->step_pool) CU(A->cuModuleGetFunction(&K->k_step_pool, K->mod, "rn_k_step_pool"));
+  if (K->traj_pool) CU(A->cuModuleGetFunction(&K->k_traj_hist, K->mod, "rn_k_traj_hist"));
   if (K->mass_pool) {
     CU(A->cuModuleGetFunction(&K->k_pool_reduce_dense, K->mod, "rn_k_pool_reduce_dense"));
     CU(A->cuModuleGetFunction(&K->k_pool_factor, K->mod, "rn_k_pool_factor"));
@@ -1127,6 +1135,10 @@ struct rn_sampler {
   std::vector<std::pair<CUevent, CUevent>> track_events;  // not yet folded into track_ms
   double track_ms = 0.0;
   int64_t chain_offset = 0;  // a restored sampler: index of its first chain in the sampler that was saved (rn_ckpt_header)
+  // pooled trajectory lengths (RN_TRAJ_POOL): the histogram over all chains of all ranks, built before the first sampling launch
+  // (or restored from a checkpoint), and on the device [bins] counts then [bins] prefix sums
+  std::vector<int64_t> traj_hist;
+  CUdeviceptr d_traj = 0;
 };
 
 namespace {
@@ -1210,6 +1222,27 @@ int iterations_to_window_end(const rn_sampler* s, int limit) {
   return limit;
 }
 
+// ---- pooled trajectory lengths (rn_config.trajectory_adaptation, definition in rainier_cuda.h) ----------------------------
+const int kTrajMaxSteps = 65536;
+uint64_t hash_words(const uint8_t* p, size_t len);  // the checkpoints' word hash (below)
+
+// the prefix sums c[l] of a histogram and its fingerprint F
+void traj_prefix(const std::vector<int64_t>& h, std::vector<int64_t>& cum, uint64_t& fp) {
+  cum.resize(h.size());
+  int64_t run = 0;
+  for (size_t l = 0; l < h.size(); l++) cum[l] = run += h[l];
+  fp = hash_words((const uint8_t*)h.data(), h.size() * 8);
+}
+// L_t (the host mirror of rn_traj_length, rn_sampler_common.cuh)
+int traj_length(const std::vector<int64_t>& cum, uint64_t fp, int64_t t) {
+  uint64_t z = fp + (uint64_t)(t + 1) * 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  z = z ^ (z >> 31);
+  const uint64_t r = (uint64_t)(((unsigned __int128)z * (uint64_t)cum.back()) >> 64);
+  return (int)(std::upper_bound(cum.begin(), cum.end(), (int64_t)r) - cum.begin());
+}
+
 // doubles of the pooled window buffer behind the arena: [2n+1]; pooled dense windows (rn_sampler_common.cuh, RN_MASS_POOL)
 // [1 + n + n^2] and the factor scratch (lower and upper packed factors, one flag)
 size_t pool_doubles(const rn_sampler* s) {
@@ -1248,6 +1281,12 @@ int check_config(const rn_model* m, const rn_config* c, int chains) {
     return fail(RN_E_INVALID, "step_adaptation must be RN_ADAPT_PER_CHAIN or RN_ADAPT_POOLED");
   if (c->step_adaptation == RN_ADAPT_POOLED && c->step_size_tuner == RN_STEP_STATIC)
     return fail(RN_E_UNSUPPORTED, "pooled step-size adaptation needs DualAvgTuner (a static step size has nothing to pool)");
+  if (c->trajectory_adaptation != RN_ADAPT_PER_CHAIN && c->trajectory_adaptation != RN_ADAPT_POOLED)
+    return fail(RN_E_INVALID, "trajectory_adaptation must be RN_ADAPT_PER_CHAIN or RN_ADAPT_POOLED");
+  if (c->trajectory_adaptation == RN_ADAPT_POOLED && c->sampler != RN_SAMPLER_EHMC)
+    return fail(RN_E_UNSUPPORTED, "pooled trajectory lengths need EHMCSampler (HMCSampler's length is fixed: nothing to pool)");
+  if (c->trajectory_adaptation == RN_ADAPT_POOLED && c->max_steps > kTrajMaxSteps)
+    return fail(RN_E_UNSUPPORTED, "pooled trajectory lengths support max_steps <= " + std::to_string(kTrajMaxSteps));
   return RN_OK;
 }
 
@@ -1578,9 +1617,53 @@ static int track_accumulate(const Api* A, rn_sampler* s, CUdeviceptr draws, int 
   return RN_OK;
 }
 
+// pooled trajectory lengths: the histogram of every chain's ring (rn_k_traj_hist), summed over ranks, unless a checkpoint
+// brought it; then its prefix sums and fingerprint go to the kernels' arguments
+static int traj_build(const Api* A, rn_sampler* s) {
+  const int bins = s->cfg.max_steps + 1;
+  if (!s->d_traj) CU(A->cuMemAlloc(&s->d_traj, (size_t)bins * 16));
+  if (s->traj_hist.empty()) {
+    CU(A->cuMemsetD8Async(s->d_traj, 0, (size_t)bins * 8, s->stream));
+    RnArgs a = s->args;
+    a.traj_hist = (rn_i64*)(uintptr_t)s->d_traj;
+    void* params[] = {&a};
+    CU(A->cuLaunchKernel(s->K->k_traj_hist, (unsigned)((s->chains + 127) / 128), 1, 1, 128, 1, 1, 0, s->stream, params, nullptr));
+    s->launches++;
+    int rc = comm_allreduce(A, s, s->d_traj, (size_t)bins, 4 /*ncclInt64*/, false);
+    if (rc) return rc;
+    std::vector<int64_t> h((size_t)bins);
+    CU(A->cuStreamSynchronize(s->stream));
+    CU(A->cuMemcpyDtoH(h.data(), s->d_traj, (size_t)bins * 8));
+    s->traj_hist = std::move(h);
+  }
+  std::vector<int64_t> cum;
+  uint64_t fp = 0;
+  traj_prefix(s->traj_hist, cum, fp);
+  CU(A->cuStreamSynchronize(s->stream));
+  CU(A->cuMemcpyHtoD(s->d_traj, s->traj_hist.data(), (size_t)bins * 8));
+  CU(A->cuMemcpyHtoD(s->d_traj + (size_t)bins * 8, cum.data(), (size_t)bins * 8));
+  RnArgs& a = s->args;
+  a.traj_hist = (rn_i64*)(uintptr_t)s->d_traj;
+  a.traj_cum = (const rn_i64*)(uintptr_t)(s->d_traj + (size_t)bins * 8);
+  a.traj_total = cum.back();
+  a.traj_fp = (rn_i64)fp;
+  a.traj_bins = bins;
+  return RN_OK;
+}
+
+// t_first: the sampling iteration of the first of these iterations (pooled trajectory lengths); -1: the next one
 static int run_phase(const Api* A, rn_sampler* s, int phase, int iterations, double* d_samples, int chain_begin = 0,
-                     int chain_end = -1) {
+                     int chain_end = -1, int64_t t_first = -1) {
   if (chain_end < 0) chain_end = s->chains;
+  if (t_first < 0) t_first = s->sampling_iterations;
+  if (phase == 1 && iterations > 0 && s->K->traj_pool && !s->args.traj_cum) {
+    // the histogram is frozen when sampling starts: the rings must be the finished warmup's
+    if (!s->initialized || s->warm_done < s->cfg.warmup_iterations)
+      return fail(RN_E_INVALID, "pooled trajectory lengths: sampling starts after the whole warmup (" + std::to_string(s->warm_done) + " of " +
+                                    std::to_string(s->cfg.warmup_iterations) + " warmup iterations done)");
+    const int rc = traj_build(A, s);
+    if (rc) return rc;
+  }
   const int per_launch = s->cfg.launch_iterations > 0 ? s->cfg.launch_iterations : 1000;
   const bool pooled = phase == 0 && s->cfg.adaptation == RN_ADAPT_POOLED &&
                       (s->cfg.mass_tuner == RN_MASS_DIAGONAL || s->cfg.mass_tuner == RN_MASS_DENSE);
@@ -1608,10 +1691,13 @@ static int run_phase(const Api* A, rn_sampler* s, int phase, int iterations, dou
     a.n_iter = k;
     a.adaptation = s->cfg.adaptation == RN_ADAPT_POOLED ? 1 : 0;
     a.tma = s->K->tma_stages > 0 ? 1 : 0;
+    a.traj_t0 = t_first + done;
     // the DMMA path wants full CTAs (8 or 16 chains): the whole groups of a batch run it, a ragged tail (and a batch that
-    // does not start on a group boundary) runs the per-warp path of the same kernel in a second launch
+    // does not start on a group boundary) runs the per-warp path of the same kernel in a second launch.  EHMC's warmup (per-chain
+    // trajectory lengths) runs all chains on that per-warp path.
     int tail_begin = chain_end;
-    if (s->K->mma) {
+    if (s->K->mma && phase == 0 && s->K->traj_pool) a.tma = 0;
+    if (s->K->mma && a.tma) {
       const int nc = s->K->mma_chains;
       if (chain_begin % nc != 0)
         a.tma = 0;
@@ -2072,6 +2158,29 @@ int rn_sampler_comm_stats(rn_sampler* s, int64_t* calls, double* total_us) {
   return RN_OK;
 }
 
+int rn_sampler_trajectory_lengths(rn_sampler* s, int64_t* counts, int cap, int* n) {
+  if (!s || !n) return fail(RN_E_INVALID, "null argument");
+  if (!s->K->traj_pool) return fail(RN_E_INVALID, "rn_sampler_trajectory_lengths: trajectory lengths are drawn per chain (trajectory_adaptation)");
+  if (s->traj_hist.empty())
+    return fail(RN_E_INVALID, "rn_sampler_trajectory_lengths: the pooled histogram is built by the first sampling launch");
+  *n = (int)s->traj_hist.size();
+  if (counts) std::memcpy(counts, s->traj_hist.data(), (size_t)std::max(0, std::min(cap, *n)) * 8);
+  return RN_OK;
+}
+
+int rn_trajectory_lengths_sequence(const int64_t* counts, int bins, int64_t t0, int64_t count, int32_t* out) {
+  if (!counts || (!out && count > 0) || bins < 1 || bins > kTrajMaxSteps + 1 || t0 < 0 || count < 0)
+    return fail(RN_E_INVALID, "rn_trajectory_lengths_sequence: bad arguments");
+  std::vector<int64_t> h(counts, counts + bins), cum;
+  for (int64_t v : h)
+    if (v < 0) return fail(RN_E_INVALID, "rn_trajectory_lengths_sequence: negative count");
+  uint64_t fp = 0;
+  traj_prefix(h, cum, fp);
+  if (cum.back() <= 0) return fail(RN_E_INVALID, "rn_trajectory_lengths_sequence: empty histogram");
+  for (int64_t k = 0; k < count; k++) out[k] = traj_length(cum, fp, t0 + k);
+  return RN_OK;
+}
+
 int rn_sampler_set_comm(rn_sampler* s, rn_comm* comm) {
   s->comm = comm;
   return RN_OK;
@@ -2102,6 +2211,7 @@ void rn_sampler_destroy(rn_sampler* s) {
     }
     if (s->d_trace) A->cuMemFree(s->d_trace);
     if (s->d_state) A->cuMemFree(s->d_state);
+    if (s->d_traj) A->cuMemFree(s->d_traj);
     if (s->d_track) A->cuMemFree(s->d_track);
     if (s->d_track_terms) A->cuMemFree(s->d_track_terms);
     if (s->d_track_sums) A->cuMemFree(s->d_track_sums);
@@ -2465,6 +2575,7 @@ int rn_sample(rn_model* m, const rn_config* cfg, const int64_t* seeds, int chain
       // block b+1 computes -- the copy, not the kernel, is the long pole of this call.
       rc = rn_sampler_run(s, 0, nullptr);  // initialize + lf.resetStats() (Driver.scala:31), no iterations
       if (rc) return rc;
+      const int64_t t_base = s->sampling_iterations;  // every chain block runs the same sampling iterations
       size_t blocks = std::min<size_t>(8, C / 32768);
       if (total < ((size_t)64 << 20)) blocks = 1;
       if (const char* e = getenv("RN_SAMPLE_BLOCKS")) blocks = (size_t)atoll(e);
@@ -2498,7 +2609,7 @@ int rn_sample(rn_model* m, const rn_config* cfg, const int64_t* seeds, int chain
         const size_t c0 = ranges[bi].first, c1 = ranges[bi].second;
         for (size_t done = 0; done < I;) {
           const size_t k = std::min(chunk, I - done);
-          rc = run_phase(A, s, 1, (int)k, (double*)(uintptr_t)g.b[0], (int)c0, (int)c1);
+          rc = run_phase(A, s, 1, (int)k, (double*)(uintptr_t)g.b[0], (int)c0, (int)c1, t_base + (int64_t)done);
           if (rc) return rc;
           rc = transpose(g.b[0] + c0 * 8, g.b[1] + c0 * I * n * 8, k, c1 - c0, I, done);
           if (rc) return rc;
@@ -3752,6 +3863,10 @@ void ckpt_header(const rn_sampler* s, const std::vector<CkptField>& L, uint64_t 
   h.step_bytes = ckpt_step_bytes(c);
   h.pool_bytes = pool_doubles(s) * 8;
   h.record_bytes = record_bytes;
+  // pooled trajectory lengths: the mode, and the byte count of the histogram that follows the pooled window buffer (0 until
+  // the first sampling launch has built it); per-chain blobs keep both 0 and are laid out as before
+  h.reserved0 = c.trajectory_adaptation;
+  h.reserved1 = (uint32_t)(s->traj_hist.size() * 8);
 }
 
 struct CkptView {  // a parsed, verified blob
@@ -3780,12 +3895,14 @@ int ckpt_parse(const void* blob, size_t len, const std::string& what, CkptView* 
                                   std::to_string(RN_CKPT_VERSION));
   if (h.header_bytes != sizeof(h) || h.n_fields > RN_STATE_MAX_FIELDS || h.chains < 1 || h.chains > INT32_MAX || h.n < 1 ||
       h.record_bytes % 8 != 0 || h.record_bytes > ((uint64_t)1 << 40) || h.step_bytes > ((uint64_t)1 << 40) ||
-      h.pool_bytes > ((uint64_t)1 << 40))
+      h.pool_bytes > ((uint64_t)1 << 40) || (h.reserved0 != RN_ADAPT_PER_CHAIN && h.reserved0 != RN_ADAPT_POOLED) ||
+      (h.reserved0 == RN_ADAPT_PER_CHAIN && h.reserved1 != 0) ||
+      (h.reserved1 != 0 && h.reserved1 != (uint64_t)(h.max_steps + 1) * 8))
     return fail(RN_E_INVALID, what + ": malformed header");
   v->p = (const uint8_t*)blob;
   v->table_off = sizeof(h);
   v->rep_off = v->table_off + (uint64_t)h.n_fields * sizeof(rn_ckpt_field);
-  v->rec_off = v->rep_off + h.step_bytes + h.pool_bytes;
+  v->rec_off = v->rep_off + h.step_bytes + h.pool_bytes + h.reserved1;
   const uint64_t records = (uint64_t)h.chains * h.record_bytes;
   if (h.record_bytes && records / h.record_bytes != (uint64_t)h.chains) return fail(RN_E_INVALID, what + ": malformed header");
   v->total = v->rec_off + records + 8;
@@ -3807,8 +3924,10 @@ int ckpt_parse(const void* blob, size_t len, const std::string& what, CkptView* 
 }
 
 // chains of a blob are independent -- may be cut apart or joined with other blobs' -- unless a pooled adaptation is still
-// warming up: pooled windows sum per rank, then over ranks, so their bits depend on how the chains are split (DESIGN.md 5)
+// warming up: pooled windows sum per rank, then over ranks, so their bits depend on how the chains are split (DESIGN.md 5).
+// With pooled trajectory lengths the chains are independent once the blob carries the histogram of all of them.
 bool ckpt_independent(const rn_ckpt_header& h) {
+  if (h.reserved0 == RN_ADAPT_POOLED && h.reserved1 == 0) return false;
   const bool pooled = h.adaptation == RN_ADAPT_POOLED || h.step_adaptation == RN_ADAPT_POOLED;
   return !pooled || (h.initialized && h.warm_done == h.warmup_iterations);
 }
@@ -3827,8 +3946,14 @@ int ckpt_same(const CkptView& a, const CkptView& b, const std::string& what) {
   RN_CKPT_SAME(initialized) RN_CKPT_SAME(warm_done) RN_CKPT_SAME(stats_reset_for_sampling) RN_CKPT_SAME(win_size)
   RN_CKPT_SAME(win_i) RN_CKPT_SAME(win_j) RN_CKPT_SAME(est_samples) RN_CKPT_SAME(mass_kind) RN_CKPT_SAME(track)
   RN_CKPT_SAME(track_thin) RN_CKPT_SAME(track_seen) RN_CKPT_SAME(track_kept) RN_CKPT_SAME(step_bytes) RN_CKPT_SAME(pool_bytes)
-  RN_CKPT_SAME(record_bytes)
+  RN_CKPT_SAME(record_bytes) RN_CKPT_SAME(reserved0) RN_CKPT_SAME(reserved1)
+  if (a.h.reserved0 == RN_ADAPT_POOLED) {  // pooled trajectory lengths: the next sampling iteration t picks L_t for every chain
+    RN_CKPT_SAME(sampling_iterations)
+  }
 #undef RN_CKPT_SAME
+  const uint64_t traj_off = a.h.step_bytes + a.h.pool_bytes;
+  if (a.h.reserved1 && std::memcmp(a.p + a.rep_off + traj_off, b.p + b.rep_off + traj_off, a.h.reserved1) != 0)
+    return fail(RN_E_INVALID, what + ": pooled trajectory-length histogram differs from the first checkpoint's");
   if (a.table.size() != b.table.size() || std::memcmp(a.table.data(), b.table.data(), a.table.size() * sizeof(rn_ckpt_field)) != 0)
     return fail(RN_E_INVALID, what + ": field table differs from the first checkpoint's");
   return RN_OK;
@@ -3847,6 +3972,9 @@ int ckpt_config_matches(const rn_ckpt_header& h, const rn_config& c) {
     RN_CKPT_CFG(warmup_iterations)
   }
 #undef RN_CKPT_CFG
+  if (h.reserved0 != c.trajectory_adaptation)
+    return fail(RN_E_INVALID, "rn_sampler_restore: rn_config.trajectory_adaptation differs (checkpoint " + std::to_string(h.reserved0) +
+                                  ", config " + std::to_string(c.trajectory_adaptation) + ")");
   return RN_OK;
 }
 
@@ -4009,8 +4137,8 @@ int rn_sampler_save(rn_sampler* s, void* buf, size_t cap, size_t* needed) {
   const std::vector<CkptField> L = ckpt_layout(s, &R);
   rn_ckpt_header h;
   ckpt_header(s, L, R, h);
-  const uint64_t table_off = sizeof(h), rep_off = table_off + L.size() * sizeof(rn_ckpt_field), rec_off = rep_off + h.step_bytes + h.pool_bytes,
-                 total = rec_off + (uint64_t)s->chains * R + 8;
+  const uint64_t table_off = sizeof(h), rep_off = table_off + L.size() * sizeof(rn_ckpt_field),
+                 rec_off = rep_off + h.step_bytes + h.pool_bytes + h.reserved1, total = rec_off + (uint64_t)s->chains * R + 8;
   if (needed) *needed = (size_t)total;
   if (!buf) return RN_OK;
   if (cap < total) return fail(RN_E_INVALID, "rn_sampler_save: buffer of " + std::to_string(cap) + " bytes, the checkpoint needs " + std::to_string(total));
@@ -4021,6 +4149,7 @@ int rn_sampler_save(rn_sampler* s, void* buf, size_t cap, size_t* needed) {
   for (size_t f = 0; f < L.size(); f++) std::memcpy(p + table_off + f * sizeof(rn_ckpt_field), &L[f].f, sizeof(rn_ckpt_field));
   CU(A->cuMemcpyDtoH(p + rep_off, s->d_step, h.step_bytes));
   CU(A->cuMemcpyDtoH(p + rep_off + h.step_bytes, s->d_pool, h.pool_bytes));
+  if (h.reserved1) std::memcpy(p + rep_off + h.step_bytes + h.pool_bytes, s->traj_hist.data(), h.reserved1);
   rc = ckpt_save_records(A, s, L, R, p + rec_off);
   if (rc) return rc;
   const uint64_t sum = blob_hash(p, total - 8);
@@ -4113,6 +4242,10 @@ int rn_sampler_restore(rn_model* m, const rn_config* cfg, const void* const* blo
   if (!same) return fail(RN_E_INVALID, "rn_sampler_restore: the checkpoint's record layout differs from this sampler's");
   CU(A->cuMemcpyHtoD(s->d_step, V[0].p + V[0].rep_off, h0.step_bytes));
   CU(A->cuMemcpyHtoD(s->d_pool, V[0].p + V[0].rep_off + h0.step_bytes, h0.pool_bytes));
+  if (h0.reserved1) {  // the pooled histogram: the next sampling launch uploads its prefix sums
+    s->traj_hist.resize(h0.reserved1 / 8);
+    std::memcpy(s->traj_hist.data(), V[0].p + V[0].rep_off + h0.step_bytes + h0.pool_bytes, h0.reserved1);
+  }
   int64_t at = 0;
   for (const CkptView& v : V) {
     rc = ckpt_load_records(A, s.get(), L, R, v.p + v.rec_off, v.h.chains, at);

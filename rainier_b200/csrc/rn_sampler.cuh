@@ -700,7 +700,13 @@ RN_DEVICE void rn_iterate(const RnArgs& A) {
         if (ring_i == A.buf_size) ring_full = 1;
         ring_i = ring_i % A.buf_size;
         RN_AT(A.ring, ring_i, c) = (double)l;
-      } else {  // steps.sample().toInt, Stats.scala:40-45
+      }
+#if RN_TRAJ_POOL
+      else if (PHASE == 1) {  // pooled: the sampling iteration's shared length, no draw (rn_sampler_common.cuh)
+        rn_take_steps(A, c, T, kind, s, rn_traj_length(A, A.traj_t0 + it), stepSize, S);
+      }
+#endif
+      else {  // steps.sample().toInt, Stats.scala:40-45
         RnRng rng = rn_rng_unpark(T);
         const int idx = ring_full ? rn_rng_int(rng, A.buf_size) : rn_rng_int(rng, ring_i + 1);
         rn_rng_park(T, rng);

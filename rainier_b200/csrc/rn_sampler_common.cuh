@@ -162,6 +162,54 @@ RN_GLOBAL void rn_k_step_pool(const RnArgs A, const rn_i64* acc, int t, int rese
 }
 #endif  // RN_STEP_POOL
 
+#ifndef RN_TRAJ_POOL
+#define RN_TRAJ_POOL 0 /* 1: pooled EHMC trajectory lengths in the sampling phase (rn_traj_length below) */
+#endif
+#if RN_TRAJ_POOL
+// ---- pooled trajectory lengths (rn_config.trajectory_adaptation == RN_ADAPT_POOLED; an extension) ------------------------
+// Warmup fills every chain's ring of U-turn counts as the reference does.  Before the first sampling launch rn_k_traj_hist
+// counts, over every chain, the ring entries steps.sample() would choose from (indices [0, ring_full ? buf_size : ring_i + 1),
+// Stats.scala:40-45) into h[l]; the host all-reduces h over ranks (int64) and uploads the prefix sums c.  Sampling iteration t
+// of every chain then takes L_t steps (the definition is in rainier_cuda.h, rn_config.trajectory_adaptation): a function of
+// the histogram and t alone, so no chain's RNG is consumed and every chain of a warp or CTA runs the same trajectory length.
+RN_GLOBAL void rn_k_traj_hist(const RnArgs A) {
+  const int c = (int)(blockIdx.x * blockDim.x + threadIdx.x);
+  if (c >= A.chains) return;
+  const int k = A.ring_full[c] ? A.buf_size : A.ring_i[c] + 1;
+  for (int i = 0; i < k; i++) {
+    const int l = rn_d2i(RN_AT(A.ring, i, c));  // 0 <= l <= max_steps (countSteps stops at maxSteps, EHMC.scala:32-50)
+#ifdef RN_HOST_EMULATION
+    __atomic_fetch_add(&A.traj_hist[l], (rn_i64)1, __ATOMIC_RELAXED);
+#else
+    atomicAdd((unsigned long long*)&A.traj_hist[l], 1ull);
+#endif
+  }
+}
+
+// L_t: z = splitmix64(F + (t + 1) * 0x9E3779B97F4A7C15), r = mulhi64(z, T), L_t = min { l : c[l] > r }.  Every thread of a warp
+// evaluates it with the same arguments, so the binary search over the prefix table is warp-uniform.
+RN_DEVICE int rn_traj_length(const RnArgs& A, rn_i64 t) {
+  unsigned long long z = (unsigned long long)A.traj_fp + (unsigned long long)(t + 1) * 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  z = z ^ (z >> 31);
+#ifdef RN_HOST_EMULATION
+  const unsigned long long r = (unsigned long long)(((unsigned __int128)z * (unsigned long long)A.traj_total) >> 64);
+#else
+  const unsigned long long r = __umul64hi(z, (unsigned long long)A.traj_total);
+#endif
+  int lo = 0, hi = A.traj_bins - 1;  // c[traj_bins - 1] = T > r
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if ((unsigned long long)A.traj_cum[mid] > r)
+      hi = mid;
+    else
+      lo = mid + 1;
+  }
+  return lo;
+}
+#endif  // RN_TRAJ_POOL
+
 #ifndef RN_HOST_EMULATION
 // =============================================================================================================
 // rn_k_transpose: [rows][cols] -> [cols][rows] (sample chunks [iter][n][chain] -> [chain][iter][n] before the

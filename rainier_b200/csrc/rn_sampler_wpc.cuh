@@ -388,7 +388,8 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
   const int slots = (int)(blockDim.x / RN_G);  // chains per CTA
   double* const stage0 = rn_smem + (((size_t)slots * RN_WPC_SMEM_DOUBLES + 15) & ~(size_t)15);
   unsigned long long* const bars = (unsigned long long*)(stage0 + (size_t)RN_TMA_STAGES * RN_TMA_TILE_DOUBLES);
-  const bool lockstep = (A.sampler == 0) && (A.tma != 0);  // HMC: every chain calls the density equally often
+  // HMC, and EHMC sampling with pooled trajectory lengths: every chain calls the density equally often
+  const bool lockstep = (A.sampler == 0 || (RN_TRAJ_POOL && A.phase == 1)) && (A.tma != 0);
   if (lockstep) {
     if (threadIdx.x == 0) {
       // RN_TMA_STAGES barriers of the CTA-shared tile pipeline, or one per warp of the chain-batched DMMA path
@@ -510,7 +511,13 @@ RN_GLOBAL void rn_k_iter(const RnArgs A) {
         ring_i = ring_i % A.buf_size;
         if (RN_LANE == 0) RN_AT(A.ring, ring_i, c) = (double)l;
         RN_SYNC();
-      } else {
+      }
+#if RN_TRAJ_POOL
+      else if (A.phase == 1) {  // pooled: the sampling iteration's shared length, no draw (rn_sampler_common.cuh)
+        rn_take_steps(A, c, w, rn_traj_length(A, A.traj_t0 + it), stepSize, S);
+      }
+#endif
+      else {
         const int idx = ring_full ? rn_rng_int(rng, A.buf_size) : rn_rng_int(rng, ring_i + 1);
         const int nsteps = rn_d2i(RN_AT(A.ring, idx, c));
         rn_take_steps(A, c, w, nsteps, stepSize, S);

@@ -23,13 +23,17 @@ import com.stripe.rainier.sampler._
   * NOT COMPILED in the rainier_b200 repository (no JVM toolchain in its build image); see INTEGRATION.md.
   */
 object CudaSampling {
-  def sample(model: Model, config: SamplerConfig = SamplerConfig.default, nChains: Int = 4, device: Int = 0)(
+  /** trajectoryAdaptation: rn_config.trajectory_adaptation (0 per chain, the reference's EHMC; 1 pooled: one shared
+    * trajectory length per sampling iteration, drawn from all chains' U-turn counts, EHMCSampler only) */
+  def sample(model: Model, config: SamplerConfig = SamplerConfig.default, nChains: Int = 4, device: Int = 0,
+             trajectoryAdaptation: Int = 0)(
       implicit rng: RNG = RNG.default,
       progress: Progress = SilentProgress): Trace = {
     val cm = CudaCompiler.compileTargets(model.targetGroup, withGradient = false, device = device)
     try {
       val n = cm.nVars
       val cfg = lower(config)
+      cfg.putInt(OffTrajAdaptation, trajectoryAdaptation)
       val seeds = Array.fill(nChains)((rng.standardUniform * (1L << 48)).toLong)
       // results land in page-locked memory (one DMA, no staging copy); read back through a DoubleBuffer view
       val sampleBytes = nChains.toLong * config.iterations * n * 8
@@ -69,7 +73,7 @@ object CudaSampling {
   private val OffBufSize = 32; private val OffPCount = 40
   private val OffStepTuner = 48; private val OffDelta = 56; private val OffStaticStep = 64
   private val OffMassTuner = 72; private val OffInitWindow = 76; private val OffExpansion = 80
-  private val OffSkipFirst = 88; private val OffSkipLast = 92
+  private val OffSkipFirst = 88; private val OffSkipLast = 92; private val OffTrajAdaptation = 100
   require(Native.configSize() == 152, "rn_config layout changed")
 
   private def lower(config: SamplerConfig): ByteBuffer = {

@@ -76,6 +76,9 @@ public final class Native {
   /** rn_sampler_tracked_diagnostics: out [n][2] = rHat, effectiveSampleSize over the tracked draws of every chain (every rank
    *  of an attached communicator calls it) */
   public static native void samplerTrackedDiagnostics(long sampler, double[] out);
+  /** rn_sampler_trajectory_lengths: the pooled histogram of U-turn counts (trajectory_adaptation = RN_ADAPT_POOLED, after the
+   *  first sampling call) into counts (null: size only); returns maxSteps + 1 */
+  public static native int samplerTrajectoryLengths(long sampler, long[] counts);
 
   /** rn_sampler_save: the staged sampler's whole state into a direct ByteBuffer (page-locked memory from hostAlloc is written by
    *  DMA); out == null returns the size only.  Returns the checkpoint's bytes */
